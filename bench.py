@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py -- the driver's measurement contract for stract_b200.
+"""bench.py -- the measurement of stract_b200's flagship workload.
 
 Headline metric (BASELINE.json): webgraph edges/sec per centrality iteration, on configs[1]
-(50M-node / 1B-edge R-MAT host graph, harmonic centrality to convergence on 1xB200; with --gpus N the
+(25M-node / 500M-edge R-MAT host graph, harmonic centrality to convergence on 1xH100 80 GB; with --gpus N the
 same graph is destination-row partitioned over N GPUs = configs[2]).  A "step" is one complete
 HarmonicCentrality computation (reset + all HyperBall iterations to convergence) on the graph
 resident in HBM; value = kept_edges x iterations / device time.  `e2e` is the same metric through the
@@ -19,6 +19,10 @@ runs on the GPU as `c1` and is checked against tests/golden/path1_c1.json.  BM25
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            our CUDA path
   python bench.py --impl reference ...                          the reference's CPU path (oracle port)
+  python bench.py --dump-outputs DIR ...                        also write the last timed step's result as DIR/*.npy
+
+The default graph is sized for one 80 GB H100: the 40 B/edge input stream and the staging temporaries of a 10^9-edge
+graph do not fit next to each other in 80 GB, 5x10^8 edges (20 GB stream, 4.4 GB resident graph, 41 GB peak while staging) do.
 """
 import argparse
 import hashlib
@@ -39,13 +43,7 @@ GOLDEN_C1 = os.path.join(ROOT, "tests", "golden", "path1_c1.json")
 
 
 def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)), "measured (MEASURED_PEAKS.json)"
-        except Exception:
-            pass
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0}, "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3 at up to 700 W), not a measured peak"
 
 
 def workload_config(nodes, edges, kept, n_nodes, iters):
@@ -53,7 +51,8 @@ def workload_config(nodes, edges, kept, n_nodes, iters):
     return {"workload": f"webgraph harmonic centrality (HyperBall) to convergence, R-MAT(0.57,0.19,0.19,0.05) {nodes} nodes / "
                         f"{edges} edges, seed 42 (BASELINE configs[1]; with --gpus N the same graph partitioned over N GPUs = configs[2])",
             "kept_edges": kept, "n_nodes": n_nodes, "iterations_per_step": iters,
-            "l2_policy": "inputs >> L2: 2 x 1.8 GB register arrays + 3.6 GB CSR per iteration, no flush needed"}
+            "l2_policy": f"inputs >> L2 (50 MB): 2 x {n_nodes * 64 / 1e9:.1f} GB register arrays + {kept * 4 / 1e9:.1f} GB CSR "
+                         "per iteration, no flush needed"}
 
 
 class ClockSampler:
@@ -144,6 +143,27 @@ def registers_checksum(regs, owned=None):
 
 def _i64(x):
     return x - (1 << 64) if x >= (1 << 63) else x
+
+
+DUMP_SAMPLE = 1 << 20   # result entries written by --dump-outputs: 6 float64 arrays of 8 MB, 48 MB in all
+
+
+def dump_outputs(out_dir, dg, stats):
+    """--dump-outputs: what a caller of the timed step receives from it -- the centrality result (ascending node id) and the
+    per-iteration changed counts -- as float64 .npy files.  The 128-bit ids go out as four exact 32-bit words.  Results
+    longer than DUMP_SAMPLE are sampled at positions drawn with a fixed seed, written to `index.npy`."""
+    import numpy as np
+    lo, hi, c = dg.result()
+    n = len(c)
+    idx = np.arange(n) if n <= DUMP_SAMPLE else np.sort(np.random.default_rng(0).choice(n, DUMP_SAMPLE, replace=False))
+    m32 = np.uint64(0xFFFFFFFF)
+    arrays = {"index": idx, "centrality": c[idx],
+              "id_lo_low32": lo[idx] & m32, "id_lo_high32": lo[idx] >> np.uint64(32),
+              "id_hi_low32": hi[idx] & m32, "id_hi_high32": hi[idx] >> np.uint64(32),
+              "n_changed_per_iteration": [s["n_changed"] for s in stats], "n_positive": [n]}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, np.float64))
 
 
 def host_threads():
@@ -332,14 +352,15 @@ def run_c1(torch, device, reps=10):
 
 
 def main():
+    global GOLDEN_C2
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--nodes", type=int, default=50_000_000)
-    ap.add_argument("--edges", type=int, default=1_000_000_000)
-    ap.add_argument("--scale", type=int, default=26)
+    ap.add_argument("--nodes", type=int, default=25_000_000)
+    ap.add_argument("--edges", type=int, default=500_000_000)
+    ap.add_argument("--scale", type=int, default=25)
     ap.add_argument("--e2e-steps", type=int, default=5)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true", help="skip the full-size oracle run (parity + cpu_baseline)")
@@ -348,15 +369,18 @@ def main():
     ap.add_argument("--no-p2p", action="store_true", help="multi-GPU: NCCL byte-max all-reduce exchange instead of the fused peer-memory stores")
     ap.add_argument("--exchange", default="auto", choices=["auto", "p2p", "symm", "multicast"],
                     help="multi-GPU fused exchange transport: CUDA IPC peer mappings, torch symmetric memory unicast, or NVSwitch "
-                         "multicast stores; auto (default) = multicast from 8 GPUs up (measured: 16.9 vs 27.0 ms per step at N = 8, "
-                         "profiles/r02_trip10_8gpu_sweep.log), CUDA IPC peer stores + device-side barrier below, and whenever the "
-                         "multicast binding is not available")
+                         "multicast stores; auto (default) = multicast from 8 GPUs up, CUDA IPC peer stores + device-side barrier "
+                         "below, and whenever the multicast binding is not available")
     ap.add_argument("--sweep", action="store_true", help="N>1: time the exchange variants (side-stream CTAs, subscriber filter, owned item "
                     "list, NVSwitch multicast) on one staged graph in one process and print one JSON line; no bench line")
     ap.add_argument("--ref-budget-s", type=float, default=170.0, help="--impl reference: wall budget of the timed loops")
     ap.add_argument("--write-golden", action="store_true", help="N=1, after a green oracle check: rewrite tests/golden/path1_c2.json")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="N=1: after the timed steps write what the last one computed as DIR/<name>.npy "
+                    "(float64; a fixed seeded sample of the centrality result, under 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -378,11 +402,13 @@ def main():
     dev = torch.device("cuda", local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
+    if args.dump_outputs and world > 1:
+        ap.error("--dump-outputs writes the result of a 1-GPU run")
     L = lib()
     peaks, peak_src = _peaks()
-    full_size = args.nodes == 50_000_000 and args.edges == 1_000_000_000 and args.scale == 26
+    gen = json.load(open(GOLDEN_C2))["generator"]
+    full_size = (args.nodes, args.edges, args.scale) == (gen["nodes"], gen["edges"], gen["scale"])
     if os.environ.get("SB200_BENCH_FINGERPRINT"):   # flow tests: compare N > 1 runs of another graph with this fingerprint file
-        global GOLDEN_C2
         GOLDEN_C2 = os.environ["SB200_BENCH_FINGERPRINT"]
         full_size = True
 
@@ -431,27 +457,15 @@ def main():
         dg.set_profiling(False)
         value = E * tot_iters / (ms_total * 1e-3)
         iters = tot_iters // args.steps
-        cap = {}
-        try:
-            cap = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        except (OSError, ValueError):
-            pass
-        same_workload = bool(cap) and cap["config"]["nodes"] == args.nodes and cap["config"]["edges"] == args.edges
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dg, stats_last)
 
         def kernel_roofline(p):
             ach = p["alg_bytes"] / (p["ms"] * 1e-3) / 1e9
-            r = {"bound": "hbm", "kernel": p["name"], "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                 "frac": ach / peaks["hbm_gbs"], "traffic": None, "dram_frac": None, "peak_source": peak_src,
-                 "launches": p["launches"], "avg_launch_ms": p["ms"] / p["launches"],
-                 "alg_bytes_per_launch": p["alg_bytes"] / p["launches"], "share_of_step": p["ms"] / ms_total}
-            c = cap.get(p["name"]) if same_workload else None
-            if c:
-                # physical twin of `frac`: DRAM bytes of the committed `ncu --set full` capture of this kernel at this
-                # workload over the launch time measured live here
-                r["traffic"] = c["dram_bytes_per_launch"]
-                r["dram_frac"] = c["dram_bytes_per_launch"] / (r["avg_launch_ms"] * 1e-3) / 1e9 / peaks["hbm_gbs"]
-                r["traffic_source"] = c.get("source", cap.get("source"))
-            return r
+            return {"bound": "hbm", "kernel": p["name"], "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
+                    "frac": ach / peaks["hbm_gbs"], "peak_source": peak_src,
+                    "launches": p["launches"], "avg_launch_ms": p["ms"] / p["launches"],
+                    "alg_bytes_per_launch": p["alg_bytes"] / p["launches"], "share_of_step": p["ms"] / ms_total}
         kern = [kernel_roofline(p) for p in prof if p["launches"]]
         dom = max((k for k in kern if "dense" in k["kernel"]), key=lambda k: k["share_of_step"], default=None)
         result.update(value=value, ms_per_step=ms_total / args.steps, iters=iters, E=E, info=info, clocks=clocks,

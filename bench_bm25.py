@@ -6,7 +6,6 @@ only ranks <= 10 000 are materialised because queries draw ranks from [10, 10 00
 uniform sorted subset drawn through geometric gaps (p = df/max_doc), tf ~ 1 + Geometric(0.6) capped at 255,
 doc length ~ LogNormal(5.5, 0.8) -> fieldnorm id.  Posting lists are written in tantivy's byte format by the
 library's host writer (sb200_postings_encode)."""
-import os
 import time
 
 import numpy as np
@@ -49,21 +48,6 @@ def log_uniform_queries(n_queries, n_terms, lo=10, hi=10_000, seed=1):
     return out - 1  # rank r is term ordinal r-1
 
 
-def _ncu(kernel, same_workload):
-    """DRAM bytes per launch and the limiter named by the committed ncu capture of this kernel at this workload
-    (profiles/ncu_traffic.json); null when there is none."""
-    import json
-    try:
-        cap = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")))["bm25"]
-        c = cap[kernel]
-    except (OSError, KeyError, ValueError):
-        return {"traffic": None}
-    if not same_workload:
-        return {"traffic": None}
-    return {"traffic": c["dram_bytes_per_launch"], "traffic_source": c.get("source", cap["source"]), "limiter": c.get("note"),
-            "ncu": {k: c[k] for k in ("l2_hit_rate_pct", "warps_active_pct", "issue_active_pct", "registers") if k in c}}
-
-
 def _alg_bytes(infos, terms, docs_scored, k_out_bytes, per_doc_bytes):
     plen = np.array([infos[i].postings_len for i in range(len(infos))], np.float64)
     return float(plen[terms].sum()) + per_doc_bytes * docs_scored + k_out_bytes
@@ -97,7 +81,7 @@ def run_and(device, peaks, max_doc=10_000_000, df_scale=2.0e6, n_queries=10_000,
                    # sparse result tables cross PCIe packed (counts, then only the filled entries) when under half of the dense table is filled
                    "d2h_bytes_per_step": int(n_queries * 4 + (8 * int(n.sum()) if 2 * int(n.sum()) < n_queries * k else n_queries * k * 8))},
            "roofline": {"bound": "hbm", "kernel": "k_and3 + k_and3_select", "achieved": alg / (kern * 1e-3) / 1e9, "peak": peaks["hbm_gbs"],
-                        "unit": "GB/s", "frac": alg / (kern * 1e-3) / 1e9 / peaks["hbm_gbs"], "alg_bytes_per_launch": alg, **_ncu("k_and3", max_doc == 10_000_000)},
+                        "unit": "GB/s", "frac": alg / (kern * 1e-3) / 1e9 / peaks["hbm_gbs"], "alg_bytes_per_launch": alg},
            "index_hbm_bytes": seg.info()["hbm_bytes"], "gen_s": round(gen_s, 1), "stage_ms": seg.info()["stage_ms"]}
     if cpu:
         out["cpu_baseline"], out["parity"] = cpu_and(ix, terms, k, seg, (d, s, n))
@@ -181,7 +165,7 @@ def run_signal(device, peaks, max_doc=100_000_000, df_scale=2.0e7, n_queries=10_
            "e2e": {"value": postings / (e2e * 1e-3), "unit": "postings/s", "ms_per_batch": e2e,
                    "h2d_bytes_per_step": int(terms.size * 8 + 1024), "d2h_bytes_per_step": int(n_queries * k * 12 + n_queries * 4)},
            "roofline": {"bound": "hbm", "kernel": "k_or3<SIGNAL,5>", "achieved": alg / (kern * 1e-3) / 1e9, "peak": peaks["hbm_gbs"],
-                        "unit": "GB/s", "frac": alg / (kern * 1e-3) / 1e9 / peaks["hbm_gbs"], "alg_bytes_per_launch": alg, **_ncu("k_or3", max_doc == 100_000_000)},
+                        "unit": "GB/s", "frac": alg / (kern * 1e-3) / 1e9 / peaks["hbm_gbs"], "alg_bytes_per_launch": alg},
            "index_hbm_bytes": seg.info()["hbm_bytes"], "gen_s": round(gen_s, 1)}
     # production-shaped variant: Stract stops a segment after max_docs_considered candidates in doc order
     # (core/src/config/defaults.rs:38-40 = 250 000; ShortCircuitQuery, tantivy/src/query/shortcircuit.rs:100-133)

@@ -1,7 +1,7 @@
-/* stract_b200.h -- C ABI of libstract_b200.so: B200-native (sm_100a) replacements for Stract's
+/* stract_b200.h -- C ABI of libstract_b200.so: H100-native (sm_90a) replacements for Stract's
  * two data-parallel ranking hot paths.  This is the drop-in boundary a Rust `extern "C"` block
  * (see INTEGRATION.md) binds; every entry point cites the reference interface it replaces
- * (paths relative to /root/reference).
+ * (paths relative to the root of the Stract repository).
  *
  * Conventions
  *   - plain pointers + sizes; the caller owns every buffer; nothing is retained after return

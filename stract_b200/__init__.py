@@ -1,4 +1,4 @@
-"""stract_b200 -- B200-native (sm_100a) replacements for Stract's two data-parallel ranking hot
+"""stract_b200 -- H100-native (sm_90a) replacements for Stract's two data-parallel ranking hot
 paths, behind a C ABI (include/stract_b200.h, libstract_b200.so) and a host-side mirror of the
 reference's interfaces:
 

@@ -45,7 +45,7 @@ extern "C" {
 
 const char* sb200_last_error(void) { return t_err; }
 #ifndef SB200_EMU
-const char* sb200_version(void) { return "stract_b200 0.1 (sm_100a)"; }
+const char* sb200_version(void) { return "stract_b200 0.1 (sm_90a)"; }
 #else
 const char* sb200_version(void) { return "stract_b200 0.1 CPU SIMT emulation (tests/emu, tests only)"; }
 #endif

@@ -1,9 +1,8 @@
 // arena.h -- host-side sub-allocator over a few large device slabs (opt-in: SB200_ARENA=1).
 //
-// Why: one sb200_graph_create at C2 size allocates and frees ~60 GB of staging temporaries.  cudaMalloc/cudaFree
-// of such sizes cost up to 150 ms apiece, and the driver's stream-ordered pool (cudaMallocAsync), which replaced
-// them, still stalls for 100-500 ms in roughly one create out of four when it has to grow or re-map
-// (profiles/r01_trip18_e2e_breakdown.log).  A create performs the same allocation sequence every time, so a
+// Why: one sb200_graph_create at C2 size allocates and frees tens of GB of staging temporaries.  cudaMalloc/cudaFree
+// of such sizes are slow, and the driver's stream-ordered pool (cudaMallocAsync), which replaced them, still stalls
+// when it has to grow or re-map.  A create performs the same allocation sequence every time, so a
 // deterministic best-fit allocator over slabs that are never returned reaches a steady state after the first
 // create and costs no driver call afterwards.
 //

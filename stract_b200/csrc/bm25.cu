@@ -852,14 +852,14 @@ static int launch_or3_occ(const WParams& P, cudaStream_t s) {
 }
 template <int MODE>
 static int launch_or3(const WParams& P, cudaStream_t s) {
-  static const int occ = [] { const char* e = getenv("SB200_OR3_OCC"); return e ? atoi(e) : 6; }();   // C5: 608 / 588 / 900 ms at 5 / 6 / 8
+  static const int occ = [] { const char* e = getenv("SB200_OR3_OCC"); return e ? atoi(e) : 6; }();
   if (occ >= 8) return launch_or3_occ<MODE, 8>(P, s);
   if (occ >= 6) return launch_or3_occ<MODE, 6>(P, s);
   return launch_or3_occ<MODE, 5>(P, s);
 }
 
 // Result tables to the caller.  An AND batch fills a fraction of its [n_queries][k] table (C4: 72 of 1000 entries per
-// query), and the dense copy of 80 MB was a third of the end-to-end time: when the tables go to host memory and are
+// query), so the dense copy of 80 MB is mostly padding: when the tables go to host memory and are
 // less than half full, the valid prefixes are packed on the device, cross PCIe as one block and are scattered into the
 // caller's tables by the host.  f32 scores only (path A); dense copy otherwise.
 __global__ void k_pack_tables(const uint32_t* __restrict__ o_n, const uint64_t* __restrict__ off, const uint32_t* __restrict__ o_docs,
@@ -975,7 +975,7 @@ static int run_and3(sb200_segment* g, const Params& P, const std::vector<uint32_
       A.units = (const AUnit*)g->a3_units.p; A.n_units = n_units;
       A.cand_off = g->a3_off.p; A.cand_cnt = g->a3_cnt.p; A.c_key = g->a3_key.p; A.c_doc = g->a3_doc.p;
       A.counters = P.counters;
-      static const int occ = [] { const char* e = getenv("SB200_AND3_OCC"); return e ? atoi(e) : 8; }();   // C4: 3.66 / 3.51 / 3.09 ms at 5 / 6 / 8
+      static const int occ = [] { const char* e = getenv("SB200_AND3_OCC"); return e ? atoi(e) : 8; }();
       if (occ >= 8) SB_LAUNCH(k_and3<8>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
       else if (occ >= 6) SB_LAUNCH(k_and3<6>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
       else SB_LAUNCH(k_and3<5>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);

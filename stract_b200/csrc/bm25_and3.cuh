@@ -1,8 +1,8 @@
-// bm25_and3.cuh -- AND queries, third generation (the default AND kernel since round 2: bit-identical to
-// k_topk_warp<AND> on hardware and 2x faster on the C4 batch; SB200_BM25_AND3=0 switches back).
+// bm25_and3.cuh -- AND queries, third generation (the default AND kernel: bit-identical to k_topk_warp<AND>;
+// SB200_BM25_AND3=0 switches back).
 //
 // Why: a CPU emulation of k_topk_warp<AND> on the C4 batch (10k 2-term queries) counts 4.1 M rounds of ~250 per
-// work item, evenly spread -- no tail -- yet the kernel needs 14 ms: ~12 us per round.  A round there is ~1500
+// work item, evenly spread -- no tail -- and a round there is ~1500
 // serial instructions of generic T-term bookkeeping on cursor structs in shared memory; the memory system is idle.
 // The intersection itself needs far less:
 //   * work unit = (query, a few consecutive 128-doc blocks of its RAREST term A); one warp per unit.  Units are
@@ -162,8 +162,7 @@ __device__ __forceinline__ float a3_term_score(float weight, uint32_t tf, float 
 }
 
 // MINB = resident CTAs per SM the register allocation aims for (5: 96 registers, no spill; 6: 80; 8: 64 with a small spill).
-// ncu on the C4 batch: 27 % warps active at 96 registers with the issue slots 47 % busy -- the kernel lives on latency
-// hiding: measured on the C4 batch 3.66 / 3.51 / 3.09 ms at MINB 5 / 6 / 8, so 8 is the default (SB200_AND3_OCC selects).
+// The kernel lives on latency hiding, so 8 is the default (SB200_AND3_OCC selects).
 template <int MINB>
 __global__ void __launch_bounds__(A3_WARPS * 32, MINB) k_and3(const A3Params P) {
   __shared__ float cache[256];

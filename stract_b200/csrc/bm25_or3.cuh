@@ -129,8 +129,8 @@ __device__ uint32_t o3_decode(const SegView& S, const uint4* __restrict__ a128, 
 }
 
 // MODE 1: OR (tantivy weights, query-order f32 sum), MODE 2: Stract BM25 + f64 linear signal combine
-// MINB: resident CTAs per SM the register allocation aims for (ncu at C5: 96 registers => 5 CTAs = 31 % of the warp slots,
-// issue slots 46 % busy, 19 of 32 lanes active: latency-bound at low occupancy; 6 => 80 registers, 8 => 64 with a small spill)
+// MINB: resident CTAs per SM the register allocation aims for (5 => 96 registers, 6 => 80, 8 => 64 with a small spill);
+// the kernel is latency-bound, so occupancy is what the choice trades against spills
 template <int MODE, int TMAX, int MINB>
 __global__ void __launch_bounds__(WQ * 32, MINB) k_or3(const WParams P) {
   static_assert(MODE == 1 || MODE == 2, "k_or3 covers the union modes");

@@ -114,8 +114,8 @@ struct DevBuf {
   }
   void adopt(T* ptr, size_t count) { release(); p = ptr; n = count; borrowed = true; }
   // Inside a PoolScope the buffer comes from the device's stream-ordered memory pool: the staging pipeline
-  // allocates and frees tens of GB of temporaries per graph, and cudaMalloc/cudaFree of such sizes cost up to
-  // ~150 ms apiece (measured as noise in the per-phase staging times); pooled memory is recycled across creates.
+  // allocates and frees tens of GB of temporaries per graph, and cudaMalloc/cudaFree of such sizes are slow;
+  // pooled memory is recycled across creates.
   int alloc(size_t count) {
     release();
     if (count == 0) { n = 0; return SB200_OK; }
@@ -151,8 +151,8 @@ static inline bool env_flag(const char* name, bool dflt) {
 
 // ---- device helpers --------------------------------------------------------------------------
 // Byte-wise unsigned max of 4 packed bytes, valid when every byte is < 128 -- which holds for HyperLogLog<64>
-// registers (rho <= 65, hyperloglog.rs:4385-4396).  sm_100a has no SIMD byte max (`__vmaxu4` is emulated with
-// ~10 LOP3/SHF/PRMT/IADD; ncu showed the pull kernels issue-bound on exactly that), so use 3 instructions:
+// registers (rho <= 65, hyperloglog.rs:4385-4396).  sm_90a has no SIMD byte max (`__vmaxu4` is emulated with
+// 6 LOP3/SHF/PRMT/IADD, and the pull kernels issue one per 4 register bytes gathered), so use 3 instructions:
 //   d = a + 0x80808080 - b   no carry/borrow crosses a byte (a_i + 0x80 <= 0xFF and >= 0x80 > b_i); MSB_i = (a_i >= b_i)
 //   m = PRMT sign-replicate  0xFF where a_i >= b_i, else 0x00
 //   r = (a & m) | (b & ~m)   one LOP3

@@ -241,9 +241,9 @@ __global__ void k_class_bounds(const uint32_t* __restrict__ deg, uint64_t n, uin
   if (d > t2 && !(nx > t2)) out[2] = i + 1;
 }
 // first row whose row_ptr >= target (rows are edge-balanced between ranks), 32-row aligned
-// Rank boundaries by estimated iteration time rather than raw edge count (measured on B200: the warp-per-item
-// kernel moves ~6.0 TB/s of algorithmic bytes, the quad-per-row kernel ~4.1 TB/s, and every row with in-edges
-// costs ~200 B of row/finalize traffic): cost(row) = 68*E_before + 34*E_quad_before + 200*min(row, n_pos).
+// Rank boundaries by estimated iteration time rather than raw edge count: 68 B per in-edge, 34 B more per in-edge of a
+// quad-per-row row (that kernel moves its bytes more slowly than the warp-per-item one), and ~200 B of row/finalize
+// traffic per row with in-edges: cost(row) = 68*E_before + 34*E_quad_before + 200*min(row, n_pos).
 __device__ __forceinline__ double split_cost(const uint32_t* row_ptr, uint64_t row, uint64_t n_warp, uint64_t n_pos) {
   const double e = (double)row_ptr[row];
   const double eq = row > n_warp ? e - (double)row_ptr[n_warp] : 0.0;
@@ -662,8 +662,8 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
     SB_TRY(sort_keys<uint64_t>(tmp, a, c, E, 0, 32 + nb, s));
     SB_LAUNCH(k_lo32, div_up(E, TPB), TPB, 0, s, a, E, col_full.p); SB_CHECK_LAUNCH();
     pt.mark("3c remap + sort (fwd CSR)");
-    // source-major CSR (single-rank handles only: the push branch needs every out-edge).  It costs a third sort
-    // (~0.2 s at 1e9 edges) and saves ~10 ms per run, so by default it is built lazily by build_fwd_csr() the first
+    // source-major CSR (single-rank handles only: the push branch needs every out-edge).  It costs a third sort of all
+    // edges and saves only the tail iterations of a run, so by default it is built lazily by build_fwd_csr() the first
     // time a REUSED handle meets a small frontier; SB200_EAGER_FWD=1 builds it here.
     if (g->world == 1 && getenv("SB200_EAGER_FWD") != nullptr) {
       uint64_t* other = c;  // scratch half of the last sort

@@ -180,8 +180,8 @@ __device__ __forceinline__ void publish_row(uint4* __restrict__ newr, uint32_t* 
   for (int p = 0; p < peers.n; p++) {
     if ((want >> peers.prank[p]) & 1u) peers.newr[p][(uint64_t)row * 4 + sub] = acc;
     // the changed bit is NOT pushed per row: a 32-row block has one owner, so k_publish_bitmap copies the owner's
-    // finished bitmap words to the peers with plain stores (3.5 M remote atomics per peer and iteration measured
-    // as the bottleneck of the 8-GPU run)
+    // finished bitmap words to the peers with plain stores (per-row remote atomics would be one per changed row,
+    // peer and iteration)
   }
 }
 
@@ -262,8 +262,8 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, 
 }
 
 // Experiment (SB200_QUAD2=1, single-rank handles): two adjacent rows per quad, their index loads and gathers interleaved --
-// twice the loads in flight per lane for the short-row class, which ncu shows waiting on the long scoreboard (69 % of the
-// DRAM peak at 87 % occupancy).  40 registers => 6 CTAs/SM instead of 7.
+// twice the loads in flight per lane for the short-row class, whose gathers wait on DRAM latency.  40 registers => 6
+// CTAs/SM instead of 7.
 template <bool FRONTIER>
 __global__ void __launch_bounds__(256, 4) k_pull_quad2(uint64_t row_begin, uint64_t row_end,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
@@ -310,7 +310,7 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad2(uint64_t row_begin, uint6
 // ---- pull, long rows: one warp per <=CHUNK_EDGES work item ---------------------------------------------
 template <bool FRONTIER, bool LISTED>
 // 8 CTAs/SM (<= 32 registers): at full scale the gathers are DRAM-latency bound and the kernel's speed tracks the
-// number of resident warps (36 registers = 7 CTAs measured 11 % slower than 32 registers = 8 CTAs)
+// number of resident warps
 __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t first_multi_free_item,
     const uint32_t* __restrict__ item_list, const uint32_t* __restrict__ item_row, const uint32_t* __restrict__ item_start, uint32_t warp_row_begin,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
@@ -586,10 +586,11 @@ int hb_alloc_state(sb200_graph* g) {
   }
   if (!g->h_counters) SB_CUDA(cudaMallocHost((void**)&g->h_counters, 8 * sizeof(unsigned long long)));
   // Rows are ordered by in-degree, so the head of the register array holds the hubs -- on a power-law graph also the
-  // most-gathered sources.  The first SB200_L2_PERSIST_MB (default 32; 0 = off) MB of the array being READ are pinned
+  // most-gathered sources.  The first SB200_L2_PERSIST_MB (default 16; 0 = off) MB of the array being READ are pinned
   // as persisting L2 lines for the pull kernels (stream access-policy window, re-pointed at the `old` array every
   // iteration), so the streaming col/row traffic cannot evict them.
-  const double mb = env_f("SB200_L2_PERSIST_MB", 32.0);  // measured at C2: 0 -> 57.5, 32 -> 54.1, 64 -> 56.2, 96 -> 60.0 ms/step
+  // H100 80 GB at 400 W, C2 (25 M ids / 500 M edges): 0 -> 53.6, 16 -> 47.9, 32 -> 67.0 ms/step (32 of the 50 MB L2 starve the streams)
+  const double mb = env_f("SB200_L2_PERSIST_MB", 16.0);
   g->l2_window_bytes = 0;
   if (mb > 0) {
     cudaDeviceProp prop;
@@ -648,8 +649,8 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
   const double per_edge = FRONTIER ? 4.0 : 68.0;  // col index (+ the 64-B gather when every source is read)
   // fused exchange: short rows on the side stream, next to the long-row kernel (see k_pull_quad_owned)
   if (g->opt_side_ctas < 0) {
-    // measured on C2 (profiles/r02_trip9_*gpu.log, r02_trip10_8gpu_sweep.log): unicast peer stores gain from the side stream at
-    // 2 and 4 ranks (35.0 -> 33.1, 22.1 -> 17.5 ms) and lose at 8 (27.0 -> 32.6 ms); one NVSwitch multicast target gains (19.5 -> 16.9)
+    // default: the side stream for up to 4 ranks and for one multicast target; with unicast stores to 7 peers the short-row
+    // kernel beside the long-row one slows both (not measured on H100: it needs several GPUs; SB200_QUAD_SIDE_CTAS overrides)
     const bool multicast_target = g->n_peers < g->world - 1;
     g->opt_side_ctas = (int)env_f("SB200_QUAD_SIDE_CTAS", (multicast_target || g->world <= 4) ? 2.0 : 0.0);
   }
@@ -922,9 +923,9 @@ int hb_step_launch(sb200_graph* g, bool with_barrier) {
   } else {
     // sharded handles: the same lazy rule for the source-major CSR (of the owned rows); every rank sees the same
     // global changed count, so all ranks switch together (SB200_SHARDED_PUSH=0 keeps them on the pull kernels)
-    // Thresholds from the 2-GPU runs on C2 (profiles/r02_trip3_2gpu.log): the iteration after 16.6 M of 27.8 M nodes changed
-    // costs 5.0 ms as a dense pull and ~3.3 ms frontier-filtered (same 0.75 N rule as a single rank without forward CSR);
-    // the one after 0.49 M changed costs 3.5 ms as a frontier pull over all local edges but < 1 ms as a push.
+    // Thresholds: below 0.75 N changed nodes a frontier-filtered pull reads fewer source registers than a dense one (the
+    // rule of a single rank without forward CSR); below N / 16 a push over the changed rows' out-edges does less work than a
+    // frontier pull, which still scans every local edge.
     static const bool auto_push = env_flag("SB200_SHARDED_PUSH", true);
     const bool tiny = (double)g->n_changed_prev * 16.0 <= (double)N;
     if (!g->has_fwd && ((auto_push && g->reuse > 0 && g->t > 0 && tiny) || force_mode == 2)) SB_TRY(build_fwd_csr(g));

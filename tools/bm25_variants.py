@@ -1,5 +1,5 @@
-"""Timing of kernel switches on one resident index (tools/gpu_r2_trip4.sh): the AND occupancy variants need a fresh process
-each (static switch), the union kernel's TMA staging toggles per call."""
+"""Timing of kernel switches on one resident index (`python tools/bm25_variants.py and|signal [scale]`): the AND occupancy
+variants need a fresh process each (static switch), the union kernel's TMA staging toggles per call."""
 import os
 import sys
 import time
