@@ -38,7 +38,7 @@ uint64_t sb200_graph::hbm_bytes() const {
   return id_lo.bytes() + id_hi.bytes() + perm.bytes() + inv.bytes() + row_ptr.bytes() + col.bytes() + fwd_ptr.bytes() +
          fwd_dst.bytes() + item_row.bytes() + item_start.bytes() + partial.bytes() + regs[0].bytes() + regs[1].bytes() +
          bm[0].bytes() + bm[1].bytes() + size_cache.bytes() + kahan_sum.bytes() + kahan_err.bytes() +
-         frontier_list.bytes() + frontier_off.bytes() + cub_tmp.bytes() + counters.bytes() + sub_mask.bytes() + sync_page.bytes();
+         frontier_list.bytes() + frontier_off.bytes() + frontier_scan.bytes() + cub_tmp.bytes() + counters.bytes() + sub_mask.bytes() + sync_page.bytes();
 }
 
 extern "C" {

@@ -62,7 +62,8 @@ struct sb200_graph {
   sb200::DevBuf<uint32_t> bm[2];
   sb200::DevBuf<uint64_t> size_cache;
   sb200::DevBuf<double> kahan_sum, kahan_err;
-  sb200::DevBuf<uint32_t> frontier_list, frontier_off;  // push mode scratch
+  sb200::DevBuf<uint32_t> frontier_list, frontier_off;  // push mode scratch: sources + their first fwd_dst index, slot offsets
+  sb200::DevBuf<unsigned long long> frontier_scan;       // push mode scratch: per bitmap word (sources << 32 | slots), + its scan
   sb200::DevBuf<uint8_t> cub_tmp;
   sb200::DevBuf<unsigned long long> counters;  // [0] n_changed [1] frontier out-edges [2..] scratch
   unsigned long long* h_counters = nullptr;    // pinned mirror

@@ -22,7 +22,8 @@
 //                     counter (4 x LDG.128), byte-wise max with __vmaxu4, xor-shuffle reduce over
 //                     the 8 quads; rows spanning several items go through a partial buffer + k_pull_merge
 //     DENSE variant gathers every in-neighbour; FRONTIER variant tests the changed bitmap first.
-//   * push kernel (source-major CSR) for small frontiers: half-warp per out-edge, 32-bit CAS max.
+//   * push kernel (source-major CSR) for small frontiers: the frontier's out-edges in equal contiguous tiles per warp,
+//     half-warp per out-edge, 32-bit CAS max.
 //   * k_finalize: per changed node, HyperLogLog<64>::size() in the reference's exact f64 operation
 //     order (sequential sum over registers 0..63, no FMA), saturating difference against the cached
 //     size(old), KahanSum update; nodes that changed in the previous iteration but not now get the
@@ -389,34 +390,63 @@ __global__ void __launch_bounds__(256) k_pull_merge(uint64_t n_rows, const uint3
 }
 
 // ---- push from a small frontier (update_changed_counters, harmonic.rs:75-114) --------------------------
-// slot_sum (sharded handles): total of the out-degrees, i.e. the number of push slots of this rank
-__global__ void k_frontier_compact(const uint32_t* __restrict__ bm, uint64_t words, const uint32_t* __restrict__ fwd_ptr,
-                                   uint32_t* list, uint32_t* outdeg, unsigned long long* counter,
-                                   unsigned long long* slot_sum) {
-  uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (w >= words) return;
-  uint32_t m = bm[w];
-  if (!m) return;
-  unsigned long long pos = atomicAdd(counter, (unsigned long long)__popc(m));
-  unsigned long long sum = 0;
+// The push SOURCES are the frontier nodes (previous iteration's changed bitmap) with at least one out-edge, listed in node
+// order; source j owns the push slots [off[j], off[j+1]), one per out-edge (of an owned destination, on a sharded handle).
+// The list is built without atomics, so it is the same every run: per bitmap word, k_frontier_count packs
+// (sources << 32 | out-edges); a CUB exclusive scan over the words gives every word its first source and first slot, and
+// k_frontier_scatter writes the list.  The halves of the packed sum never carry into each other: the slot total is at most
+// E < 2^32 (fwd_ptr is u32).  A frontier node without out-edges is not a source, so every source has >= 1 slot (k_push
+// relies on it).
+__global__ void k_frontier_count(const uint32_t* __restrict__ bm, uint64_t words, const uint32_t* __restrict__ fwd_ptr,
+                                 unsigned long long* __restrict__ word_sum) {
+  const uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (w > words) return;
+  uint32_t m = w < words ? bm[w] : 0u;   // entry `words` is 0: its scanned value is the total
+  uint32_t n = 0, d = 0;
   while (m) {
-    int b = __ffs(m) - 1; m &= m - 1;
-    uint32_t v = (uint32_t)(w * 32 + b);
-    const uint32_t d = fwd_ptr[v + 1] - fwd_ptr[v];
-    list[pos] = v; outdeg[pos] = d; pos++; sum += d;
+    const uint32_t v = (uint32_t)(w * 32 + (__ffs(m) - 1));
+    m &= m - 1;
+    const uint32_t dv = fwd_ptr[v + 1] - fwd_ptr[v];
+    n += dv != 0u; d += dv;
   }
-  if (slot_sum && sum) atomicAdd(slot_sum, sum);
+  word_sum[w] = ((unsigned long long)n << 32) | d;
 }
-// refresh the two-iteration-old rows of the frontier nodes; a sharded handle refreshes the rows it owns (the others
-// arrive from their owners)
-__global__ void k_copy_stale(const uint32_t* __restrict__ list, uint64_t n, const uint4* __restrict__ oldr,
+// slot_total (sharded handles): the number of push slots of this rank, for the host
+__global__ void k_frontier_scatter(const uint32_t* __restrict__ bm, uint64_t words, const uint32_t* __restrict__ fwd_ptr,
+                                   const unsigned long long* __restrict__ word_pos, uint32_t* __restrict__ list,
+                                   uint32_t* __restrict__ fbeg, uint32_t* __restrict__ off, unsigned long long* slot_total) {
+  const uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (w > words) return;
+  const unsigned long long p = word_pos[w];
+  uint32_t j = (uint32_t)(p >> 32), o = (uint32_t)p;
+  if (w == words) {   // off[n_sources] = slot total
+    off[j] = o;
+    if (slot_total) *slot_total = o;
+    return;
+  }
+  uint32_t m = bm[w];
+  while (m) {
+    const uint32_t v = (uint32_t)(w * 32 + (__ffs(m) - 1));
+    m &= m - 1;
+    const uint32_t f0 = fwd_ptr[v], dv = fwd_ptr[v + 1] - f0;
+    if (!dv) continue;
+    list[j] = v; fbeg[j] = f0; off[j] = o;
+    j++; o += dv;
+  }
+}
+// refresh the two-iteration-old rows of the frontier nodes; one quad per bitmap word.  A sharded handle refreshes the rows
+// it owns (whole bitmap words, see owned_row); the others arrive from their owners.
+__global__ void k_copy_stale(const uint32_t* __restrict__ bm, uint64_t words, const uint4* __restrict__ oldr,
                              uint4* __restrict__ newr, uint32_t world, uint32_t rank) {
-  uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  uint64_t i = gt >> 2;
-  if (i >= n) return;
-  uint64_t v = list[i];
-  if (world > 1 && ((v >> 5) % world) != rank) return;
-  newr[v * 4 + (gt & 3)] = oldr[v * 4 + (gt & 3)];
+  const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const uint64_t w = (gt >> 2) * world + rank;   // this rank's k-th bitmap word
+  if (w >= words) return;
+  uint32_t m = __ldg(bm + w);
+  while (m) {
+    const uint64_t v = w * 32 + (uint64_t)(__ffs(m) - 1);
+    m &= m - 1;
+    newr[v * 4 + (gt & 3)] = oldr[v * 4 + (gt & 3)];
+  }
 }
 // fused exchange after a push: every owned row that was refreshed or changed in this iteration goes to the peers
 // (the frontier is small by construction: one quad per OWNED bitmap word, i.e. per 32-row block, walks the set bits)
@@ -435,33 +465,86 @@ __global__ void k_publish_rows(const uint32_t* __restrict__ bm_prev, const uint3
     for (int p = 0; p < peers.n; p++) if ((want >> peers.prank[p]) & 1u) peers.newr[p][row * 4 + (gt & 3)] = v;
   }
 }
-__global__ void __launch_bounds__(256) k_push(const uint32_t* __restrict__ list, const uint32_t* __restrict__ off,
-    uint32_t n_front, uint64_t n_slots, const uint32_t* __restrict__ fwd_ptr, const uint32_t* __restrict__ fwd_dst,
+// Load-balanced push.  The slots are cut into one contiguous tile per warp (a multiple of 32 slots), so a source with many
+// out-edges spreads over several warps and every warp gets the same work.  A warp finds the source of its first slot with
+// one binary search over `off`, then walks its tile 32 slots at a time:
+//   * the lanes load the window of sources cur .. cur+31 (list, fbeg, off: coalesced).  The 32 slots of a chunk lie in at
+//     most 32 sources, because every source has >= 1 slot; each lane finds its slot's source by a 5-step search over the
+//     shuffled window ends and loads its destination (consecutive slots of one source read consecutive fwd_dst words);
+//   * each half-warp then takes every other slot: one 64-B row, 16 lanes x 4 B.  The source row stays in registers while
+//     consecutive slots share the source; PUSH_BATCH destination rows are loaded and their first CAS issued before any
+//     result is waited for, so several rows per half-warp are in flight.  The byte max is a 32-bit CAS loop (bmax4_7bit);
+//     a destination that changed gets its bit in bm_cur.
+// `total` = the scanned (sources << 32 | slots) of the whole frontier (the last entry of the scan): the source count is
+// known only on the device.
+constexpr int PUSH_BATCH = 4;
+constexpr int PUSH_CTAS_PER_SM = 6;   // 40 registers without spills
+__global__ void __launch_bounds__(256, PUSH_CTAS_PER_SM) k_push(const unsigned long long* __restrict__ total, const uint32_t* __restrict__ list,
+    const uint32_t* __restrict__ fbeg, const uint32_t* __restrict__ off, const uint32_t* __restrict__ fwd_dst,
     const uint32_t* __restrict__ old32, uint32_t* new32, uint32_t* __restrict__ bm_cur) {
-  const uint32_t lane = threadIdx.x & 31, l = lane & 15;
-  const uint64_t hw = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 4;
-  const uint64_t nhw = ((uint64_t)gridDim.x * blockDim.x) >> 4;
-  for (uint64_t s = hw; s < ((n_slots + 1) & ~1ull); s += nhw) {  // both halves of a warp iterate together
-    bool changed = false;
-    uint32_t v = 0;
-    if (s < n_slots) {
-      uint32_t lo = 0, hi = n_front;  // last j with off[j] <= s
-      while (lo + 1 < hi) { uint32_t mid = (lo + hi) >> 1; if (off[mid] <= s) lo = mid; else hi = mid; }
-      const uint32_t u = list[lo];
-      v = fwd_dst[fwd_ptr[u] + (uint32_t)(s - off[lo])];
-      const uint32_t mine = old32[(uint64_t)u * 16 + l];
-      uint32_t* addr = new32 + (uint64_t)v * 16 + l;
-      uint32_t cur = *addr;
-      uint32_t m = bmax4_7bit(cur, mine);
-      while (m != cur) {
-        const uint32_t prev = atomicCAS(addr, cur, m);
-        if (prev == cur) { changed = true; break; }
-        cur = prev; m = bmax4_7bit(cur, mine);
+  const unsigned long long tot = *total;
+  const uint32_t n_src = (uint32_t)(tot >> 32), n_slots = (uint32_t)tot;
+  const uint32_t lane = threadIdx.x & 31, l = lane & 15, half = lane >> 4;
+  const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  const uint64_t warp = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
+  const uint64_t tile = ((n_slots + n_warps - 1) / n_warps + 31) & ~31ull;
+  if (warp * tile >= n_slots) return;   // whole warp
+  const uint32_t s0 = (uint32_t)(warp * tile), s1 = (uint32_t)min(warp * tile + tile, (uint64_t)n_slots);
+  uint32_t lo = 0, hi = n_src;   // cur = last source j with off[j] <= s0
+  while (lo + 1 < hi) { const uint32_t mid = (lo + hi) >> 1; if (off[mid] <= s0) lo = mid; else hi = mid; }
+  uint32_t cur = lo;
+  uint32_t row_u = 0xFFFFFFFFu, row = 0;   // this half-warp's source row
+  for (uint32_t S = s0; S < s1; S += 32) {
+    const uint32_t wj = min(cur + lane, n_src - 1);
+    const uint32_t w_end = off[min(cur + lane + 1, n_src)];   // end of source cur+lane (the slot total past the last one)
+    const uint32_t w_beg = off[wj], w_u = list[wj], w_f = fbeg[wj];
+    const uint32_t s = S + lane;
+    uint32_t k = 0;   // number of window sources that end at or before slot s: its source is cur + k (k <= 31)
+#pragma unroll
+    for (uint32_t step = 16; step; step >>= 1) {
+      const uint32_t e = __shfl_sync(0xffffffffu, w_end, k + step - 1);
+      if (e <= s) k += step;
+    }
+    const uint32_t u = __shfl_sync(0xffffffffu, w_u, k);
+    const uint32_t e_first = __shfl_sync(0xffffffffu, w_f, k) + (s - __shfl_sync(0xffffffffu, w_beg, k));
+    const uint32_t n_here = min(32u, s1 - S);
+    const uint32_t v = lane < n_here ? ld_stream_u32(fwd_dst + e_first) : 0u;
+    cur += __popc(__ballot_sync(0xffffffffu, w_end <= S + 32));   // source of slot S + 32
+    for (uint32_t p0 = 0; p0 < n_here; p0 += 2 * PUSH_BATCH) {
+      uint32_t dst[PUSH_BATCH], mine[PUSH_BATCH], old[PUSH_BATCH], want[PUSH_BATCH], got[PUSH_BATCH];
+      bool live[PUSH_BATCH];
+#pragma unroll
+      for (int q = 0; q < PUSH_BATCH; q++) {
+        const uint32_t from = p0 + 2 * q + half;   // lane holding this half-warp's q-th slot
+        const uint32_t uq = __shfl_sync(0xffffffffu, u, from);
+        dst[q] = __shfl_sync(0xffffffffu, v, from);
+        live[q] = from < n_here;
+        if (live[q] && uq != row_u) { row = __ldg(old32 + (uint64_t)uq * 16 + l); row_u = uq; }
+        mine[q] = row;
+      }
+#pragma unroll
+      for (int q = 0; q < PUSH_BATCH; q++) old[q] = live[q] ? new32[(uint64_t)dst[q] * 16 + l] : 0u;
+#pragma unroll
+      for (int q = 0; q < PUSH_BATCH; q++) {
+        want[q] = live[q] ? bmax4_7bit(old[q], mine[q]) : old[q];
+        got[q] = want[q] != old[q] ? atomicCAS(new32 + (uint64_t)dst[q] * 16 + l, old[q], want[q]) : old[q];
+      }
+#pragma unroll
+      for (int q = 0; q < PUSH_BATCH; q++) {
+        bool changed = want[q] != old[q] && got[q] == old[q];
+        if (want[q] != old[q] && !changed) {   // another push got there first: retry against its value
+          uint32_t* addr = new32 + (uint64_t)dst[q] * 16 + l;
+          uint32_t c = got[q], m = bmax4_7bit(c, mine[q]);
+          while (m != c) {
+            const uint32_t prev = atomicCAS(addr, c, m);
+            if (prev == c) { changed = true; break; }
+            c = prev; m = bmax4_7bit(c, mine[q]);
+          }
+        }
+        const unsigned ball = __ballot_sync(0xffffffffu, changed);
+        if (((ball >> (16 * half)) & 0xFFFFu) && l == 0) atomicOr(bm_cur + (dst[q] >> 5), 1u << (dst[q] & 31));
       }
     }
-    const unsigned ball = __ballot_sync(0xffffffffu, changed);
-    const unsigned half = (lane < 16) ? (ball & 0xFFFFu) : (ball >> 16);
-    if (half && l == 0) atomicOr(bm_cur + (v >> 5), 1u << (v & 31));
   }
 }
 
@@ -736,12 +819,26 @@ static int run_push(sb200_graph* g, const uint4* oldr, uint4* newr, const uint32
   const uint64_t N = g->N, words = (N + 31) / 32;
   const uint64_t nf = g->n_changed_prev;
   if (nf == 0) return SB200_OK;  // empty frontier: a converged state is a fixed point
-  if (g->frontier_list.n < nf + 1) { SB_TRY(g->frontier_list.alloc(nf + 1 + (nf >> 2))); }
-  if (g->frontier_off.n < 2 * (nf + 1)) { SB_TRY(g->frontier_off.alloc(2 * (nf + 1) + (nf >> 1))); }
-  uint32_t* outdeg = g->frontier_off.p + (g->frontier_off.n / 2);
-  SB_CUDA(cudaMemsetAsync(g->counters.p + 2, 0, 2 * sizeof(unsigned long long), s));
-  SB_LAUNCH(k_frontier_compact, div_up(words, 256), 256, 0, s, bmp, words, g->fwd_ptr.p, g->frontier_list.p, outdeg,
-            g->counters.p + 2, g->world > 1 ? g->counters.p + 3 : (unsigned long long*)nullptr);
+  // the frontier's node count bounds the number of sources
+  if (g->frontier_list.n < 2 * (nf + 1)) { SB_TRY(g->frontier_list.alloc(2 * (nf + 1) + (nf >> 1))); }
+  if (g->frontier_off.n < nf + 1) { SB_TRY(g->frontier_off.alloc(nf + 1 + (nf >> 2))); }
+  if (g->frontier_scan.n < 2 * (words + 1)) { SB_TRY(g->frontier_scan.alloc(2 * (words + 1))); }
+  uint32_t* list = g->frontier_list.p;
+  uint32_t* fbeg = g->frontier_list.p + g->frontier_list.n / 2;
+  unsigned long long* word_sum = g->frontier_scan.p;
+  unsigned long long* word_pos = g->frontier_scan.p + (words + 1);
+  SB_LAUNCH(k_frontier_count, div_up(words + 1, 256), 256, 0, s, bmp, words, g->fwd_ptr.p, word_sum);
+  SB_CHECK_LAUNCH();
+  size_t need = 0;
+  SB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, need, word_sum, word_pos, (int64_t)(words + 1), s));
+  if (g->cub_tmp.n < need) SB_TRY(g->cub_tmp.alloc(need + 256));
+  SB_CUDA(cub::DeviceScan::ExclusiveSum(g->cub_tmp.p, need, word_sum, word_pos, (int64_t)(words + 1), s));
+  g_launches.fetch_add(2, std::memory_order_relaxed);
+  SB_LAUNCH(k_frontier_scatter, div_up(words + 1, 256), 256, 0, s, bmp, words, g->fwd_ptr.p, word_pos, list, fbeg,
+            g->frontier_off.p, g->world > 1 ? g->counters.p + 3 : (unsigned long long*)nullptr);
+  SB_CHECK_LAUNCH();
+  SB_LAUNCH(k_copy_stale, div_up(div_up(words, (uint64_t)g->world) * 4, 256), 256, 0, s, bmp, words, oldr, newr,
+            (uint32_t)g->world, (uint32_t)g->rank);
   SB_CHECK_LAUNCH();
   uint64_t slots = g->frontier_edges_prev;
   if (g->world > 1) {   // this rank's share of the frontier's out-edges is not known from the previous step
@@ -750,18 +847,13 @@ static int run_push(sb200_graph* g, const uint4* oldr, uint4* newr, const uint32
     SB_CUDA(cudaStreamSynchronize(s));
     slots = h;
   }
-  size_t need = 0;
-  SB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, need, outdeg, g->frontier_off.p, (int64_t)nf, s));
-  if (g->cub_tmp.n < need) SB_TRY(g->cub_tmp.alloc(need + 256));
-  SB_CUDA(cub::DeviceScan::ExclusiveSum(g->cub_tmp.p, need, outdeg, g->frontier_off.p, (int64_t)nf, s));
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  SB_LAUNCH(k_copy_stale, div_up(nf * 4, 256), 256, 0, s, g->frontier_list.p, nf, oldr, newr, (uint32_t)g->world, (uint32_t)g->rank);
-  SB_CHECK_LAUNCH();
   if (slots) {
-    unsigned grid = (unsigned)std::min<uint64_t>(div_up(slots * 16, 256), 148u * 16u);
+    // one wave of resident CTAs, and at least 32 slots per warp
+    if (!g->sm_count) SB_CUDA(cudaDeviceGetAttribute(&g->sm_count, cudaDevAttrMultiProcessorCount, g->device));
+    const unsigned grid = (unsigned)std::min<uint64_t>(div_up(slots, 32 * 8), (uint64_t)g->sm_count * PUSH_CTAS_PER_SM);
     PROF_BEGIN(g, sb200_graph::F_PUSH);
-    SB_LAUNCH(k_push, grid, 256, 0, s, g->frontier_list.p, g->frontier_off.p, (uint32_t)nf, slots, g->fwd_ptr.p,
-              g->fwd_dst.p, (const uint32_t*)oldr, (uint32_t*)newr, bmc);
+    SB_LAUNCH(k_push, grid, 256, 0, s, word_pos + words, list, fbeg, g->frontier_off.p, g->fwd_dst.p,
+              (const uint32_t*)oldr, (uint32_t*)newr, bmc);
     SB_CHECK_LAUNCH();
     PROF_END(g, sb200_graph::F_PUSH, 132.0 * (double)slots);
   }
