@@ -37,7 +37,7 @@ using namespace sb200;
 uint64_t sb200_graph::hbm_bytes() const {
   return id_lo.bytes() + id_hi.bytes() + perm.bytes() + inv.bytes() + row_ptr.bytes() + col.bytes() + fwd_ptr.bytes() +
          fwd_dst.bytes() + item_row.bytes() + item_start.bytes() + partial.bytes() + regs[0].bytes() + regs[1].bytes() +
-         bm[0].bytes() + bm[1].bytes() + size_cache.bytes() + kahan_sum.bytes() + kahan_err.bytes() +
+         seed.bytes() + bm[0].bytes() + bm[1].bytes() + size_cache.bytes() + kahan_sum.bytes() + kahan_err.bytes() +
          frontier_list.bytes() + frontier_off.bytes() + frontier_scan.bytes() + cub_tmp.bytes() + counters.bytes() + sub_mask.bytes() + sync_page.bytes();
 }
 
@@ -196,7 +196,8 @@ int sb200_hyperball_set_profiling(sb200_graph* g, int on) {
 int sb200_hyperball_get_profile(sb200_graph* g, sb200_kernel_prof* out, uint32_t cap, uint32_t* n) {
   if (!g || !n) SB_FAIL(SB200_EINVAL, "NULL argument");
   static const char* names[sb200_graph::F_COUNT] = {"k_pull_warp<dense>", "k_pull_quad<dense>", "k_pull_warp<frontier>",
-                                                     "k_pull_quad<frontier>", "k_pull_merge", "k_push", "k_finalize"};
+                                                     "k_pull_quad<frontier>", "k_pull_merge", "k_push", "k_finalize",
+                                                     "k_pull_warp<seed>", "k_pull_quad<seed>"};
   uint32_t k = 0;
   for (int f = 0; f < sb200_graph::F_COUNT; f++) {
     if (out && k < cap) {

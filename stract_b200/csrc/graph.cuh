@@ -8,6 +8,7 @@
 //   col          [E_local] u32 source (internal) of every kept in-edge 4 B/edge
 //   fwd_ptr/fwd_dst           source-major CSR for small frontiers     4 B/edge + 4 B/node
 //   regs[2]      [N][64] u8   HyperLogLog<64> registers, ping-pong     128 B/node
+//   seed         [N] u16      the one non-zero register of every reset counter, j | p << 8 (iteration 0 reads these)  2 B/node
 //   bm[2]        [N/32] u32   changed bitmaps (previous / current)     2 bit/node
 //   size_cache   [N] u64      size(old[v])                             8 B/node
 //   kahan_sum/err[N] f64      KahanSum per node                        16 B/node
@@ -59,6 +60,7 @@ struct sb200_graph {
 
   // iteration state
   sb200::DevBuf<uint8_t> regs[2];
+  sb200::DevBuf<uint16_t> seed;   // written by hb_reset with the registers; every rank of a sharded handle holds all N
   sb200::DevBuf<uint32_t> bm[2];
   sb200::DevBuf<uint64_t> size_cache;
   sb200::DevBuf<double> kahan_sum, kahan_err;
@@ -94,7 +96,8 @@ struct sb200_graph {
   uint64_t l2_window_bytes = 0;  // SB200_L2_PERSIST_MB: persisting-L2 access window over the hot prefix of the `old` register array
 
   // optional per-kernel-family device timing (bench evidence; CUDA events on this handle's stream)
-  enum { F_PULL_WARP_DENSE, F_PULL_QUAD_DENSE, F_PULL_WARP_FRONT, F_PULL_QUAD_FRONT, F_PULL_MERGE, F_PUSH, F_FINALIZE, F_COUNT };
+  enum { F_PULL_WARP_DENSE, F_PULL_QUAD_DENSE, F_PULL_WARP_FRONT, F_PULL_QUAD_FRONT, F_PULL_MERGE, F_PUSH, F_FINALIZE,
+         F_PULL_WARP_SEED, F_PULL_QUAD_SEED, F_COUNT };
   bool profiling = false;
   uint64_t prof_launches[F_COUNT] = {0};
   double prof_ms[F_COUNT] = {0}, prof_bytes[F_COUNT] = {0};

@@ -21,7 +21,8 @@
 //                     indices of a batch are loaded coalesced, each quad of lanes gathers one 64-B
 //                     counter (4 x LDG.128), byte-wise max with __vmaxu4, xor-shuffle reduce over
 //                     the 8 quads; rows spanning several items go through a partial buffer + k_pull_merge
-//     DENSE variant gathers every in-neighbour; FRONTIER variant tests the changed bitmap first.
+//     DENSE variant gathers every in-neighbour; FRONTIER variant tests the changed bitmap first; SEED variant (iteration
+//     0) gathers every in-neighbour's 2-B seed instead of its 64-B row: a reset counter has one non-zero register.
 //   * push kernel (source-major CSR) for small frontiers: the frontier's out-edges in equal contiguous tiles per warp,
 //     half-warp per out-edge, 32-bit CAS max.
 //   * k_finalize: per changed node, HyperLogLog<64>::size() in the reference's exact f64 operation
@@ -29,7 +30,8 @@
 //     size(old), KahanSum update; nodes that changed in the previous iteration but not now get the
 //     reference's "+= 0.0" (it is idempotent after one application, so skipping the other N-1 zero
 //     adds is bit-exact).
-// Roofline: HBM.  Algorithmic bytes per iteration: 68 B x E_active + 132 B x N_written + 40 B x N_changed.
+// Roofline: HBM.  Algorithmic bytes per iteration: 68 B x E_active + 132 B x N_written + 40 B x N_changed
+// (iteration 0: 6 B per edge instead of 68, the index and a 2-B seed).
 #include <chrono>
 #include "graph.cuh"
 #include "../../include/sb200_hll_tables.h"
@@ -128,8 +130,17 @@ __device__ __forceinline__ void kahan_add(double& sum, double& err, double rhs) 
 }
 
 // ---- init: counters seeded with the node's own id (low 64 bits), harmonic.rs:53-73 ------------------
+// A freshly seeded counter has one non-zero register: j = hash >> 58 holds p = clz(hash << 6) + 1 (1..65).  The seed
+// j | p << 8 is all of it, and iteration 0 reads 2 B per source instead of 64 (see the SEED pull variants).
+// seed_slice expands a seed into the 16-B slice `sub` of its row (registers 16 sub .. 16 sub + 15).
+__device__ __forceinline__ uint4 seed_slice(uint32_t s, uint32_t sub) {
+  const uint32_t j = s & 63u;
+  const uint32_t v = ((j >> 4) == sub) ? (s >> 8) << (8 * (j & 3u)) : 0u;
+  const uint32_t w = (j >> 2) & 3u;
+  return make_uint4(w == 0u ? v : 0u, w == 1u ? v : 0u, w == 2u ? v : 0u, w == 3u ? v : 0u);
+}
 __global__ void k_hb_init(const uint64_t* __restrict__ id_lo, const uint32_t* __restrict__ perm, uint64_t N,
-                          uint4* r0, uint4* r1, uint64_t* size_cache, double* ksum, double* kerr) {
+                          uint4* r0, uint4* r1, uint16_t* seed, uint64_t* size_cache, double* ksum, double* kerr) {
   __shared__ HllTables tab;
   for (int i = threadIdx.x; i < (int)(sizeof(HllTables) / 8); i += blockDim.x) ((double*)&tab)[i] = ((const double*)&c_tab)[i];
   __syncthreads();
@@ -139,15 +150,14 @@ __global__ void k_hb_init(const uint64_t* __restrict__ id_lo, const uint32_t* __
   const uint32_t j = (uint32_t)(hash >> 58);
   const uint64_t wv = hash << 6;
   const uint32_t p = (wv == 0 ? 64u : (uint32_t)__clzll((long long)wv)) + 1u;
+  const uint32_t s = j | p << 8;
+  seed[v] = (uint16_t)s;
   uint32_t w[16];
 #pragma unroll
-  for (int i = 0; i < 16; i++) w[i] = 0;
-#pragma unroll
-  for (int i = 0; i < 16; i++) if ((int)(j >> 2) == i) w[i] = p << (8 * (j & 3));
-#pragma unroll
   for (int q = 0; q < 4; q++) {
-    uint4 x = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+    const uint4 x = seed_slice(s, (uint32_t)q);
     r0[v * 4 + q] = x; r1[v * 4 + q] = x;
+    w[4 * q] = x.x; w[4 * q + 1] = x.y; w[4 * q + 2] = x.z; w[4 * q + 3] = x.w;
   }
   size_cache[v] = hll64_size(w, &tab);
   ksum[v] = 0.0; kerr[v] = 0.0;
@@ -191,13 +201,16 @@ __device__ __forceinline__ bool bm_test(const uint32_t* __restrict__ bm, uint32_
 }
 
 // ---- pull, short rows: 4 lanes per destination row ----------------------------------------------------
-template <bool FRONTIER>
+// SEED (iteration 0 only, see hb_step_launch): every row of `oldr` is the one-hot row of its seed, so the own row and
+// the sources are built from seed[] (2 B per source, L2-resident) and `oldr` is not read.
+template <bool FRONTIER, bool SEED>
 __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub, uint32_t lane,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
-    const uint4* __restrict__ oldr, uint4* __restrict__ newr,
+    const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut& peers) {
+  static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
   const uint32_t e0 = live ? row_ptr[row] - col_base : 0u, e1 = live ? row_ptr[row + 1] - col_base : 0u;
-  const uint4 own = oldr[row * 4 + sub];
+  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub) : oldr[row * 4 + sub];
   uint4 acc = own;
   // lane `sub` fetches source index e+sub (one 16-B request per quad per 4 edges, prefetched one step ahead)
   // and the quad shares the four indices by shuffle; an out-of-range or (FRONTIER) unchanged source is
@@ -205,6 +218,23 @@ __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub,
   const unsigned qmask = 0xFu << (lane & ~3u);
   const uint32_t self = (uint32_t)row;
   uint32_t nxt = (e0 + sub < e1) ? ld_stream_u32(col + e0 + sub) : self;
+  if (SEED) {
+    // the seed of step k is loaded during step k-1 and the index of step k+1 with it, so that one seed and one index
+    // load per lane are in flight while the quad folds in the previous four seeds
+    uint32_t sn = __ldg(seed + nxt);
+    nxt = (e0 + 4 + sub < e1) ? ld_stream_u32(col + e0 + 4 + sub) : self;
+    for (uint32_t e = e0; e < e1; e += 4) {
+      const uint32_t mine = sn;
+      sn = __ldg(seed + nxt);
+      nxt = (e + 8 + sub < e1) ? ld_stream_u32(col + e + 8 + sub) : self;
+      const uint32_t s0 = __shfl_sync(qmask, mine, 0, 4);
+      const uint32_t s1 = __shfl_sync(qmask, mine, 1, 4);
+      const uint32_t s2 = __shfl_sync(qmask, mine, 2, 4);
+      const uint32_t s3 = __shfl_sync(qmask, mine, 3, 4);
+      acc = vmax_u8x16(vmax_u8x16(acc, seed_slice(s0, sub)),
+                       vmax_u8x16(vmax_u8x16(seed_slice(s1, sub), seed_slice(s2, sub)), seed_slice(s3, sub)));
+    }
+  } else
   for (uint32_t e = e0; e < e1; e += 4) {
     uint32_t mine = nxt;
     nxt = (e + 4 + sub < e1) ? ld_stream_u32(col + e + 4 + sub) : self;
@@ -225,10 +255,10 @@ __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub,
   publish_row(newr, bm_cur, peers, (uint32_t)row, sub, acc, changed || bm_test(bm_prev, (uint32_t)row), changed);
 }
 
-template <bool FRONTIER>
+template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64_t row_end,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
-    const uint4* __restrict__ oldr, uint4* __restrict__ newr,
+    const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
   const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   const uint32_t sub = threadIdx.x & 3;
@@ -238,17 +268,17 @@ __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64
   if (!live) row = row_end - 1;  // keep the warp converged; results of dead quads are discarded
   live = live && owned_row(peers, (uint32_t)row);
   if (__ballot_sync(0xffffffffu, live) == 0u) return;  // none of this warp's rows belongs to this rank
-  quad_rows<FRONTIER>(row, live, sub, lane, row_ptr, col, col_base, oldr, newr, bm_prev, bm_cur, peers);
+  quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, col_base, oldr, seed, newr, bm_prev, bm_cur, peers);
 }
 
 // Sharded handles with the fused exchange: the short rows are most of the rows, so this kernel carries most of the
 // stores into the peers' replicas -- it is bound by NVLink, not by HBM, while k_pull_warp is the opposite.  This variant
 // is a small persistent grid (a few CTAs per SM) that walks the OWNED 32-row blocks only (4 warps per block), so that it can
 // sit next to k_pull_warp on a second, higher-priority stream: link traffic of the short rows under the gathers of the long ones.
-template <bool FRONTIER>
+template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, uint64_t row_end, uint64_t first_block, uint64_t n_tasks,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
-    const uint4* __restrict__ oldr, uint4* __restrict__ newr,
+    const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
   const uint32_t sub = threadIdx.x & 3, lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
@@ -258,7 +288,7 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, 
     const bool live = row >= row_begin && row < row_end;
     if (!live) row = row_begin;
     if (__ballot_sync(0xffffffffu, live) == 0u) continue;
-    quad_rows<FRONTIER>(row, live, sub, lane, row_ptr, col, col_base, oldr, newr, bm_prev, bm_cur, peers);
+    quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, col_base, oldr, seed, newr, bm_prev, bm_cur, peers);
   }
 }
 
@@ -309,14 +339,15 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad2(uint64_t row_begin, uint6
 }
 
 // ---- pull, long rows: one warp per <=CHUNK_EDGES work item ---------------------------------------------
-template <bool FRONTIER, bool LISTED>
+template <bool FRONTIER, bool LISTED, bool SEED>
 // 8 CTAs/SM (<= 32 registers): at full scale the gathers are DRAM-latency bound and the kernel's speed tracks the
 // number of resident warps
 __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t first_multi_free_item,
     const uint32_t* __restrict__ item_list, const uint32_t* __restrict__ item_row, const uint32_t* __restrict__ item_start, uint32_t warp_row_begin,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
-    const uint4* __restrict__ oldr, uint4* __restrict__ newr, uint4* __restrict__ partial,
+    const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr, uint4* __restrict__ partial,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
+  static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
   uint64_t item = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
   if (item >= n_items) return;  // whole warp exits together
   if (LISTED) item = item_list[item];   // sharded: n_items counts the owned items, listed ascending
@@ -331,6 +362,23 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
   // out-of-range lanes and (FRONTIER) unchanged sources are redirected to the row itself: merging one's own row
   // is a no-op under max and hits L1, so the gather loop is branch-free
   uint32_t nxt = (e0 + lane < e1) ? ld_stream_u32(col + e0 + lane) : row;
+  if (SEED) {
+    // SEED (see quad_rows): each lane loads the 2-B seed of its source, one batch ahead, and the index one batch
+    // further; each quad then takes four of the 32 seeds by shuffle and folds in their slices
+    uint32_t sn = __ldg(seed + nxt);
+    nxt = (e0 + 32 + lane < e1) ? ld_stream_u32(col + e0 + 32 + lane) : row;
+    for (uint32_t base = e0; base < e1; base += 32) {
+      const uint32_t mine = sn;
+      sn = __ldg(seed + nxt);
+      nxt = (base + 64 + lane < e1) ? ld_stream_u32(col + base + 64 + lane) : row;
+      const uint32_t s0 = __shfl_sync(0xffffffffu, mine, q);
+      const uint32_t s1 = __shfl_sync(0xffffffffu, mine, q + 8);
+      const uint32_t s2 = __shfl_sync(0xffffffffu, mine, q + 16);
+      const uint32_t s3 = __shfl_sync(0xffffffffu, mine, q + 24);
+      acc = vmax_u8x16(vmax_u8x16(acc, seed_slice(s0, sub)),
+                       vmax_u8x16(vmax_u8x16(seed_slice(s1, sub), seed_slice(s2, sub)), seed_slice(s3, sub)));
+    }
+  } else
   for (uint32_t base = e0; base < e1; base += 32) {
     uint32_t mine = nxt;
     nxt = (base + 32 + lane < e1) ? ld_stream_u32(col + base + 32 + lane) : row;
@@ -356,14 +404,15 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
     if (q == 0) partial[item * 4 + sub] = acc;
     return;
   }
-  const uint4 own = oldr[(uint64_t)row * 4 + sub];
+  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub) : oldr[(uint64_t)row * 4 + sub];
   acc = vmax_u8x16(acc, own);
   const unsigned ball = __ballot_sync(0xffffffffu, ne_u4(acc, own));
   const bool changed = (ball & 0xFu) != 0u;
   if (q == 0) publish_row(newr, bm_cur, peers, row, sub, acc, changed || bm_test(bm_prev, row), changed);
 }
 
-// rows spanning several work items: one warp reduces the parked partials
+// rows spanning several work items: one warp reduces the parked partials (the own row comes from `oldr` in the seed
+// iteration too: it equals the seed's row then, and these are a few rows)
 __global__ void __launch_bounds__(256) k_pull_merge(uint64_t n_rows, const uint32_t* __restrict__ item_start,
     uint32_t warp_row_begin, const uint4* __restrict__ partial, const uint4* __restrict__ oldr,
     uint4* __restrict__ newr, const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
@@ -658,6 +707,7 @@ int hb_alloc_state(sb200_graph* g) {
   SB_TRY(load_tables(g->device));
   SB_TRY(g->regs[0].alloc(std::max<uint64_t>(N, 1) * 64));
   SB_TRY(g->regs[1].alloc(std::max<uint64_t>(N, 1) * 64));
+  SB_TRY(g->seed.alloc(std::max<uint64_t>(N, 1)));
   SB_TRY(g->bm[0].alloc(words + 1)); SB_TRY(g->bm[1].alloc(words + 1));
   SB_TRY(g->size_cache.alloc(std::max<uint64_t>(N, 1)));
   SB_TRY(g->kahan_sum.alloc(std::max<uint64_t>(N, 1))); SB_TRY(g->kahan_err.alloc(std::max<uint64_t>(N, 1)));
@@ -673,6 +723,9 @@ int hb_alloc_state(sb200_graph* g) {
   // as persisting L2 lines for the pull kernels (stream access-policy window, re-pointed at the `old` array every
   // iteration), so the streaming col/row traffic cannot evict them.
   // H100 80 GB at 400 W, C2 (25 M ids / 500 M edges): 0 -> 53.6, 16 -> 47.9, 32 -> 67.0 ms/step (32 of the 50 MB L2 starve the streams)
+  // The seed iteration (t = 0) points the window at the seed array instead, capped at the same size.  Iteration 0 of C2
+  // (28.8 MB of seeds), same card: no window 6.87, 16 MB 6.93, the whole array (SB200_L2_PERSIST_MB=30) 6.18 ms -- but a
+  // 30 MB set-aside slows the dense iterations from 8.4 to 10.3 ms, so the cap stays.
   const double mb = env_f("SB200_L2_PERSIST_MB", 16.0);
   g->l2_window_bytes = 0;
   if (mb > 0) {
@@ -694,7 +747,7 @@ int hb_reset(sb200_graph* g) {
   g->n_changed_prev = N; g->frontier_edges_prev = g->E_kept;
   if (N == 0) return SB200_OK;
   SB_LAUNCH(k_hb_init, div_up(N, 256), 256, 0, s, g->id_lo.p, g->perm.p, N, (uint4*)g->regs[0].p, (uint4*)g->regs[1].p,
-            g->size_cache.p, g->kahan_sum.p, g->kahan_err.p);
+            g->seed.p, g->size_cache.p, g->kahan_sum.p, g->kahan_err.p);
   SB_CHECK_LAUNCH();
   SB_LAUNCH(k_bm_fill, div_up(words, 256), 256, 0, s, g->bm[0].p, N, words);  // changed_nodes filled, harmonic.rs:223-225
   SB_CHECK_LAUNCH();
@@ -723,13 +776,30 @@ static PeerOut make_peer_out(const sb200_graph* g, bool with_targets) {
   return po;
 }
 
-template <bool FRONTIER>
+// persisting-L2 access-policy window of the pull kernels on stream `s` (see hb_alloc_state)
+static int set_l2_window(cudaStream_t s, const void* base, uint64_t bytes) {
+  cudaStreamAttrValue a;
+  memset(&a, 0, sizeof(a));
+  a.accessPolicyWindow.base_ptr = (void*)base; a.accessPolicyWindow.num_bytes = bytes;
+  a.accessPolicyWindow.hitRatio = 1.0f; a.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+  a.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+  SB_CUDA(cudaStreamSetAttribute(s, cudaStreamAttributeAccessPolicyWindow, &a));
+  return SB200_OK;
+}
+// the window of a pull: the head of the `old` array, or in the seed iteration the head of the seed array
+static void l2_window_of(const sb200_graph* g, const uint4* oldr, bool from_seed, const void** base, uint64_t* bytes) {
+  *base = from_seed ? (const void*)g->seed.p : (const void*)oldr;
+  *bytes = from_seed ? std::min<uint64_t>(g->l2_window_bytes, g->N * sizeof(uint16_t)) : g->l2_window_bytes;
+}
+
+template <bool FRONTIER, bool SEED>
 static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uint32_t* bmp, uint32_t* bmc) {
   cudaStream_t s = g->stream;
   const PeerOut po = make_peer_out(g, true);
-  const int FW = FRONTIER ? sb200_graph::F_PULL_WARP_FRONT : sb200_graph::F_PULL_WARP_DENSE;
-  const int FQ = FRONTIER ? sb200_graph::F_PULL_QUAD_FRONT : sb200_graph::F_PULL_QUAD_DENSE;
-  const double per_edge = FRONTIER ? 4.0 : 68.0;  // col index (+ the 64-B gather when every source is read)
+  const int FW = SEED ? sb200_graph::F_PULL_WARP_SEED : FRONTIER ? sb200_graph::F_PULL_WARP_FRONT : sb200_graph::F_PULL_WARP_DENSE;
+  const int FQ = SEED ? sb200_graph::F_PULL_QUAD_SEED : FRONTIER ? sb200_graph::F_PULL_QUAD_FRONT : sb200_graph::F_PULL_QUAD_DENSE;
+  // per edge: the col index, + the 64-B gather when every source is read, or + its 2-B seed in the seed iteration
+  const double per_edge = SEED ? 6.0 : FRONTIER ? 4.0 : 68.0;
   // fused exchange: short rows on the side stream, next to the long-row kernel (see k_pull_quad_owned)
   if (g->opt_side_ctas < 0) {
     // default: the side stream for up to 4 ranks and for one multicast target; with unicast stores to 7 peers the short-row
@@ -756,19 +826,17 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
     SB_CUDA(cudaEventRecord(g->ev_fork, s));
     SB_CUDA(cudaStreamWaitEvent(g->side_stream, g->ev_fork, 0));
     if (g->l2_window_bytes) {
-      cudaStreamAttrValue a;
-      memset(&a, 0, sizeof(a));
-      a.accessPolicyWindow.base_ptr = (void*)oldr; a.accessPolicyWindow.num_bytes = g->l2_window_bytes;
-      a.accessPolicyWindow.hitRatio = 1.0f; a.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-      a.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-      SB_CUDA(cudaStreamSetAttribute(g->side_stream, cudaStreamAttributeAccessPolicyWindow, &a));
+      const void* wbase; uint64_t wbytes;
+      l2_window_of(g, oldr, SEED, &wbase, &wbytes);
+      SB_TRY(set_l2_window(g->side_stream, wbase, wbytes));
     }
     if (g->profiling) SB_CUDA(cudaEventRecord(g->side_prof[0], g->side_stream));
     if (getenv("SB200_DEBUG_SIDE")) fprintf(stderr, "[sb200] side quad: rank %d tasks %llu\n", g->rank, (unsigned long long)n_tasks);
     if (n_tasks) {
       const unsigned grid = (unsigned)std::min<uint64_t>(div_up(n_tasks, 8), (uint64_t)sm_count * (uint64_t)side_ctas);
-      SB_LAUNCH(k_pull_quad_owned<FRONTIER>, grid, 256, 0, g->side_stream, g->quad_row_begin, g->quad_row_end, first, n_tasks,
-                g->row_ptr.p, g->col.p, g->col_base, oldr, newr, bmp, bmc, po);
+      auto kern = k_pull_quad_owned<FRONTIER, SEED>;
+      SB_LAUNCH(kern, grid, 256, 0, g->side_stream, g->quad_row_begin, g->quad_row_end, first, n_tasks,
+                g->row_ptr.p, g->col.p, g->col_base, oldr, g->seed.p, newr, bmp, bmc, po);
       SB_CHECK_LAUNCH();
     }
     if (g->profiling) {
@@ -782,11 +850,11 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
     if (g->opt_owned_list < 0) g->opt_owned_list = env_flag("SB200_OWNED_ITEMS", true) ? 1 : 0;
     const bool listed = g->opt_owned_list > 0 && g->world > 1 && g->owned_items.p;
     const uint64_t n_launch = listed ? g->n_owned_items : g->n_items;
-    auto kern = listed ? k_pull_warp<FRONTIER, true> : k_pull_warp<FRONTIER, false>;
+    auto kern = listed ? k_pull_warp<FRONTIER, true, SEED> : k_pull_warp<FRONTIER, false, SEED>;
     if (n_launch)
     SB_LAUNCH(kern, div_up(n_launch * 32, 256), 256, 0, s, n_launch, g->n_multi_items,
-              listed ? g->owned_items.p : (const uint32_t*)nullptr, g->item_row.p, g->item_start.p, (uint32_t)g->warp_row_begin, g->row_ptr.p, g->col.p, g->col_base, oldr, newr,
-              g->partial.p, bmp, bmc, po);
+              listed ? g->owned_items.p : (const uint32_t*)nullptr, g->item_row.p, g->item_start.p, (uint32_t)g->warp_row_begin, g->row_ptr.p, g->col.p, g->col_base, oldr,
+              g->seed.p, newr, g->partial.p, bmp, bmc, po);
     SB_CHECK_LAUNCH();
     PROF_END(g, FW, g->own_frac * (per_edge * (double)g->E_warp + 68.0 * (double)(g->warp_row_end - g->warp_row_begin - g->n_multi_rows)));
   }
@@ -802,12 +870,13 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
   else if (nq) {
     PROF_BEGIN(g, FQ);
     static const bool quad2 = env_flag("SB200_QUAD2", false);
-    if (quad2 && g->world == 1 && g->col_base == 0)
+    auto kern = k_pull_quad<FRONTIER, SEED>;
+    if (quad2 && !SEED && g->world == 1 && g->col_base == 0)
       SB_LAUNCH(k_pull_quad2<FRONTIER>, div_up(((nq + 1) / 2) * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
                 g->col.p, oldr, newr, bmp, bmc);
     else
-    SB_LAUNCH(k_pull_quad<FRONTIER>, div_up(nq * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
-              g->col.p, g->col_base, oldr, newr, bmp, bmc, po);
+    SB_LAUNCH(kern, div_up(nq * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
+              g->col.p, g->col_base, oldr, g->seed.p, newr, bmp, bmc, po);
     SB_CHECK_LAUNCH();
     PROF_END(g, FQ, g->own_frac * (per_edge * (double)g->E_quad + 68.0 * (double)nq));
   }
@@ -1031,16 +1100,19 @@ int hb_step_launch(sb200_graph* g, bool with_barrier) {
   // at the END of the previous step (before the inter-step barrier), never at the start of this one
   if (!g->p2p) SB_CUDA(cudaMemsetAsync(bmc, 0, (words + 1) * 4, s));
   SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 8 * sizeof(unsigned long long), s));
+  // Iteration 0 pulls from the seeds.  Invariant: at t = 0 every row of regs[cur] is the one-hot row of its seed --
+  // hb_reset writes both from one hash (create and bind_state end in hb_reset), and no call writes registers between
+  // a reset and the first step.  bm_prev is all ones at t = 0, so a forced frontier pull is the same pull; a forced
+  // push keeps its path.
+  const bool from_seed = g->t == 0 && mode != 2;
   if (g->l2_window_bytes && mode != 2) {
-    cudaStreamAttrValue a;
-    memset(&a, 0, sizeof(a));
-    a.accessPolicyWindow.base_ptr = (void*)oldr; a.accessPolicyWindow.num_bytes = g->l2_window_bytes;
-    a.accessPolicyWindow.hitRatio = 1.0f; a.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    a.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    SB_CUDA(cudaStreamSetAttribute(s, cudaStreamAttributeAccessPolicyWindow, &a));
+    const void* wbase; uint64_t wbytes;
+    l2_window_of(g, oldr, from_seed, &wbase, &wbytes);
+    SB_TRY(set_l2_window(s, wbase, wbytes));
   }
-  if (mode == 0) SB_TRY(launch_pull<false>(g, oldr, newr, bmp, bmc));
-  else if (mode == 1) SB_TRY(launch_pull<true>(g, oldr, newr, bmp, bmc));
+  if (from_seed) SB_TRY((launch_pull<false, true>(g, oldr, newr, bmp, bmc)));
+  else if (mode == 0) SB_TRY((launch_pull<false, false>(g, oldr, newr, bmp, bmc)));
+  else if (mode == 1) SB_TRY((launch_pull<true, false>(g, oldr, newr, bmp, bmc)));
   else SB_TRY(run_push(g, oldr, newr, bmp, bmc));
   if (g->p2p && g->n_peers > 0) {
     const PeerOut po = make_peer_out(g, true);
