@@ -210,6 +210,57 @@ SB200_API int sb200_postings_encode(const uint32_t* docs, const uint32_t* tfs, c
 SB200_API int sb200_postings_encode_ex(const uint32_t* docs, const uint32_t* tfs, const uint64_t* term_off, uint32_t n_terms,
                                        const uint8_t* fieldnorm_ids, uint32_t max_doc, float avg_fieldnorm, int record_option,
                                        uint8_t* out, uint64_t out_cap, uint64_t* out_len, sb200_term_info* infos, int threads);
+/* ---- positions and phrase queries (tantivy path A for PhraseQuery) ------------------------------------------------------
+ * Host-side PositionSerializer (tantivy/src/positions/serializer.rs:47-87) for synthetic / test segments.  Input is CSR by
+ * term and posting: term t owns postings [term_off[t], term_off[t+1]); posting p owns tfs[p] absolute, ascending positions,
+ * concatenated in posting order in `positions`.  Each posting's positions become deltas (the first one against 0, u32
+ * arithmetic like the recorder), 128 deltas are one compress_block_unsorted block, the rest of a term is a VInt tail.  The
+ * output is the field's `.pos` bytes and every term's byte range.  Call with out == NULL to get the byte size. */
+SB200_API int sb200_positions_encode(const uint32_t* positions, const uint32_t* tfs, const uint64_t* term_off, uint32_t n_terms,
+                                     uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* positions_off,
+                                     uint64_t* positions_len);
+/* Attaches a field's positions file (PositionReader, tantivy/src/positions/reader.rs) to a segment opened with
+ * SB200_RECORD_FREQS_POSITIONS: copies the bytes into HBM and builds, on the device, the byte offset of every bit-packed
+ * positions block and the position offset of every posting block (the prefix of the skip entries' term-frequency sums,
+ * tantivy/src/postings/skip.rs:219,261-266).  positions_off / positions_len [n_terms] are the terms' byte ranges in the file
+ * (TermInfo.positions_range).  A segment with another record option is rejected with SB200_EINVAL (PhraseQuery's
+ * SchemaError, phrase_query.rs:106-118); ranges outside the file, malformed VInt headers or tails and bit widths > 32 with
+ * SB200_EFORMAT.  Attaching again replaces the previous positions. */
+SB200_API int sb200_segment_attach_positions(sb200_segment* seg, const uint8_t* positions_file, uint64_t len,
+                                             const uint64_t* positions_off, const uint64_t* positions_len);
+/* PositionReader::read on the device decoder: the n position DELTAS [offset, offset + n) of term `term` into `out` (host or
+ * device).  SB200_ERANGE when the term has fewer positions. */
+SB200_API int sb200_positions_read(sb200_segment* seg, uint32_t term, uint64_t offset, uint32_t n, uint32_t* out);
+/* TermInfo.positions_range of every ordinal of a TermInfoStore (term_info_store.rs:63-91), next to
+ * sb200_term_info_store_decode: positions_off / positions_len receive min(cap, n) entries, *n_terms the number of terms. */
+SB200_API int sb200_term_info_store_decode_positions(const uint8_t* store, uint64_t len, int device, uint64_t* positions_off,
+                                                     uint64_t* positions_len, uint64_t cap, uint64_t* n_terms);
+
+#define SB200_ABSENT_TERM 0xFFFFFFFEu  /* a phrase term the segment does not hold: the phrase matches nothing (phrase_weight.rs:53-61) */
+/* A batch of phrase queries over one field (PhraseWeight -> PhraseScorer -> TopNComputer).  Row q holds the phrase's terms
+ * in offset order (PhraseQuery::new_with_offset_and_slop sorts them stably by offset), then SB200_NO_TERM padding; a row
+ * has 2..SB200_MAX_QUERY_TERMS terms.  Duplicate terms are separate cursors.  The library intersects them in tantivy's
+ * Intersection order (stable sort by doc_freq) and verifies every candidate's positions:
+ *   scoring != 0  count = PhraseScorer::compute_phrase_count, match = count > 0,
+ *                 score = weight[q] * (count / (count + tf_cache256[fieldnorm_id]))   (f32, bm25.rs:182-196)
+ *   scoring == 0  match = PhraseScorer::phrase_exists, score = 1.0                   (EnableScoring::Disabled)
+ * top-k by (score desc, doc asc). */
+typedef struct {
+  uint32_t n_queries, n_terms;  /* n_terms = row width */
+  const uint32_t* term_ords;    /* [n_queries*n_terms] */
+  const uint32_t* offsets;      /* [n_queries*n_terms] position offset of each term; NULL = 0, 1, 2, ... */
+  const uint32_t* slop;         /* [n_queries]; NULL = 0 */
+  const float* weights;         /* [n_queries] Bm25Weight::for_terms(...).weight; read when scoring != 0 */
+  const float* tf_cache256;     /* [256]; read when scoring != 0 */
+  int scoring;
+  uint32_t k;
+} sb200_phrase_batch;
+/* candidates: documents holding every term; matches: candidates whose positions match; positions_decoded / position_bytes:
+ * position deltas decoded and bytes of the position blocks and tails they come from; ms / kernel_ms as sb200_bm25_stats. */
+typedef struct { uint64_t candidates, matches, positions_decoded, position_bytes; float ms, kernel_ms; } sb200_phrase_stats;
+SB200_API int sb200_phrase_topk_batch(sb200_segment* seg, const sb200_phrase_batch* batch, uint32_t* docs, float* scores,
+                                      uint32_t* n_out, sb200_phrase_stats* stats);
+
 /* idf(doc_freq, doc_count) = ln(1 + (N - n + 0.5) / (n + 0.5)) in f32 (tantivy/src/query/bm25.rs:52-56,
  * core/src/ranking/bm25.rs:23-27) for an array of doc_freqs; tantivy_weight != 0 returns Bm25Weight.weight = idf * (1 + K1). */
 SB200_API int sb200_bm25_idf(const uint32_t* doc_freq, uint64_t n, uint64_t doc_count, int tantivy_weight, float* out);

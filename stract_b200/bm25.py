@@ -8,6 +8,7 @@ Mirrors (same names / argument meaning):
   SegmentReader.open                        InvertedIndexReader + FieldNormReader of one field
   TopDocs.with_limit(k) + BooleanQuery      tantivy/src/collector/top_score_collector.rs:360-414
   SignalComputer (one text field + numeric signals)   core/src/ranking/computer/mod.rs, initial.rs:79-93
+  PhraseQuery + TopDocs.search_phrase_batch  tantivy/src/query/phrase_query (positions attached to the SegmentReader)
 
 The weights are computed on the host exactly like the reference does before it opens any posting list
 (f32 `ln` once per term); all per-posting work runs in the CUDA library.
@@ -25,6 +26,7 @@ K1 = np.float32(1.2)
 B_ = np.float32(0.75)
 MODE_AND, MODE_OR, MODE_OR_WAND = 0, 1, 2   # MODE_OR_WAND: block_wand replayed, bit-exact sums for >= 3 terms
 NO_TERM = 0xFFFFFFFF
+ABSENT_TERM = 0xFFFFFFFE   # a phrase term the segment does not hold
 
 
 def id_to_fieldnorm(i):
@@ -94,6 +96,18 @@ class Bm25Weight:
     def for_one_term(cls, term_doc_freq, total_num_docs, avg_fieldnorm):
         return cls(idf(term_doc_freq, total_num_docs), avg_fieldnorm)
 
+    @classmethod
+    def for_terms(cls, term_doc_freqs, total_num_docs, avg_fieldnorm):
+        """bm25.rs:98-134: one term is for_one_term; several sum their idf in f32 in the order given (a PhraseQuery's
+        terms in offset order)."""
+        dfs = [int(d) for d in term_doc_freqs]
+        if len(dfs) == 1:
+            return cls.for_one_term(dfs[0], total_num_docs, avg_fieldnorm)
+        idf_sum = np.float32(0.0)
+        for d in dfs:
+            idf_sum = np.float32(idf_sum + idf(d, total_num_docs))
+        return cls(idf_sum, avg_fieldnorm)
+
     def score(self, fieldnorm_id, term_freq):
         tf = np.float32(term_freq)
         return np.float32(self.weight * (tf / (tf + self.cache[fieldnorm_id])))
@@ -144,6 +158,34 @@ def encode_postings_csr(docs, tfs, off, fieldnorm_ids, avg_fieldnorm, threads=8,
     return out[:ln.value], infos
 
 
+def encode_positions(positions, tfs, term_off):
+    """PositionSerializer for a whole field (sb200_positions_encode).  CSR input: term t owns postings
+    [term_off[t], term_off[t+1]), posting p owns tfs[p] absolute ascending positions, concatenated in `positions`.
+    Returns (the `.pos` bytes u8[], positions_off u64[n_terms], positions_len u64[n_terms])."""
+    L = lib()
+    pos = np.ascontiguousarray(positions, np.uint32); tf = np.ascontiguousarray(tfs, np.uint32)
+    off = np.ascontiguousarray(term_off, np.uint64)
+    n = off.size - 1
+    ln = C.c_uint64(0)
+    check(L.sb200_positions_encode(_p(pos), _p(tf), _p(off), n, None, 0, C.byref(ln), None, None))
+    out = np.zeros(max(ln.value, 1), np.uint8)
+    po = np.zeros(max(n, 1), np.uint64); pl = np.zeros(max(n, 1), np.uint64)
+    check(L.sb200_positions_encode(_p(pos), _p(tf), _p(off), n, _p(out), out.size, C.byref(ln), _p(po), _p(pl)))
+    return out[:ln.value], po[:n], pl[:n]
+
+
+def decode_term_info_store_positions(store, device=0):
+    """TermInfo.positions_range of every ordinal of a TermInfoStore (sb200_term_info_store_decode_positions):
+    returns (positions_off u64[n], positions_len u64[n])."""
+    L = lib()
+    store = np.ascontiguousarray(store, np.uint8)
+    n = C.c_uint64(0)
+    check(L.sb200_term_info_store_decode_positions(_p(store), store.size, device, None, None, 0, C.byref(n)))
+    po = np.zeros(max(n.value, 1), np.uint64); pl = np.zeros(max(n.value, 1), np.uint64)
+    check(L.sb200_term_info_store_decode_positions(_p(store), store.size, device, _p(po), _p(pl), n.value, C.byref(n)))
+    return po[:n.value], pl[:n.value]
+
+
 def decode_term_info_store(store, device=0):
     """TermInfoStore bytes (the `.term` store behind tantivy's FST term dictionary) -> TermInfo array, decoded on the
     device (sb200_term_info_store_decode); pass the result to SegmentReader."""
@@ -159,7 +201,10 @@ def decode_term_info_store(store, device=0):
 class SegmentReader:
     """One field of one segment resident in HBM (postings file + fieldnorms + block directory)."""
 
-    def __init__(self, postings, term_infos, fieldnorm_ids, device=0, record_option=1, total_num_tokens=None):
+    def __init__(self, postings, term_infos, fieldnorm_ids, device=0, record_option=1, total_num_tokens=None, positions=None,
+                 positions_ranges=None):
+        """`positions` / `positions_ranges` = the field's `.pos` bytes and (positions_off, positions_len) per term: attached
+        when given (record_option must be 2), which enables phrase queries."""
         self._L = lib()
         self._h = C.c_void_p()
         postings = np.ascontiguousarray(postings, np.uint8)
@@ -191,6 +236,21 @@ class SegmentReader:
         # average_fieldnorm = total_num_tokens as f32 / total_num_docs as f32 (bm25.rs:112-114)
         self.average_fieldnorm = np.float32(np.float32(total_num_tokens) / np.float32(max(self.max_doc, 1)))
         self.device = device
+        if positions is not None:
+            self.attach_positions(positions, positions_ranges)
+
+    def attach_positions(self, positions, positions_ranges):
+        """sb200_segment_attach_positions: `positions_ranges` = (positions_off, positions_len) per term."""
+        pos = np.ascontiguousarray(positions, np.uint8)
+        po = np.ascontiguousarray(positions_ranges[0], np.uint64); pl = np.ascontiguousarray(positions_ranges[1], np.uint64)
+        assert po.size == self.n_terms and pl.size == self.n_terms, "one positions range per term"
+        check(self._L.sb200_segment_attach_positions(self._h, _p(pos), pos.size, _p(po), _p(pl)))
+
+    def read_positions(self, term, offset, n):
+        """PositionReader::read on the device: the n position deltas [offset, offset + n) of `term`."""
+        out = np.zeros(max(int(n), 1), np.uint32)
+        check(self._L.sb200_positions_read(self._h, int(term), int(offset), int(n), _p(out)))
+        return out[:int(n)]
 
     def info(self):
         si = B.SegmentInfo()
@@ -346,6 +406,38 @@ class TopDocs:
             return docs, scores, n_out, {k_: getattr(st, k_) for k_, _ in B.Bm25Stats._fields_ if not k_.startswith("_")}
         return docs, scores, n_out
 
+    def search_phrase_batch(self, segment, term_ords, offsets=None, slop=None, scoring=True, weights=None, average_fieldnorm=None,
+                            return_stats=False):
+        """Phrase queries over one segment (PhraseWeight::for_each_pruning -> PhraseScorer -> TopNComputer).
+        term_ords [n_queries, n_terms]: each row a phrase's terms in offset order (see PhraseQuery.rows), NO_TERM pads the end,
+        ABSENT_TERM marks a term the segment does not hold.  offsets (same shape, default 0, 1, 2, ...) and slop [n_queries]
+        as PhraseQuery::new_with_offset_and_slop.  scoring=False is EnableScoring::Disabled: every match scores 1.0.
+        `weights` [n_queries] (Bm25Weight::for_terms(..).weight) / `average_fieldnorm` override the segment's own statistics.
+        Returns (docs [nq,k], scores [nq,k], n_out [nq])."""
+        term_ords = np.ascontiguousarray(term_ords, np.uint32)
+        nq, nt = term_ords.shape
+        avg = segment.average_fieldnorm if average_fieldnorm is None else np.float32(average_fieldnorm)
+        if scoring and weights is None:
+            held = term_ords < segment.n_terms
+            df = np.where(held, segment.doc_freq[np.minimum(term_ords, max(segment.n_terms - 1, 0))], 0)
+            weights = [Bm25Weight.for_terms(df[q][term_ords[q] != NO_TERM], segment.max_doc, avg).weight for q in range(nq)]
+        w = np.ascontiguousarray(weights if weights is not None else np.zeros(nq), np.float32)
+        offs = None if offsets is None else np.ascontiguousarray(offsets, np.uint32)
+        sl = None if slop is None else np.ascontiguousarray(np.broadcast_to(np.asarray(slop, np.uint32), (nq,)))
+        cache = compute_tf_cache(avg)
+        k = self.limit + self.offset
+        docs = host_out((nq, k), np.uint32); scores = host_out((nq, k), np.float32); n_out = np.zeros(nq, np.uint32)
+        b = B.PhraseBatch(nq, nt, _p(term_ords), _p(offs), _p(sl), _p(w), _p(cache), 1 if scoring else 0, k)
+        st = B.PhraseStats()
+        check(segment._L.sb200_phrase_topk_batch(segment._h, C.byref(b), _p(docs), _p(scores), _p(n_out), C.byref(st)))
+        if self.offset:
+            o = self.offset
+            docs = np.ascontiguousarray(docs[:, o:]); scores = np.ascontiguousarray(scores[:, o:])
+            n_out = (np.maximum(n_out.astype(np.int64) - o, 0)).astype(np.uint32)
+        if return_stats:
+            return docs, scores, n_out, {k_: getattr(st, k_) for k_, _ in B.PhraseStats._fields_}
+        return docs, scores, n_out
+
     def search(self, segment, term_ords, mode=MODE_AND, weights=None):
         """One query -> list of (score, doc) like the Fruit Vec<(Score, DocAddress)>."""
         t = np.asarray(term_ords, np.uint32)[None, :]
@@ -407,6 +499,63 @@ class Searcher:
             m = order.size
             out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = segs[order], docs[order], scs[order], m
         return out_seg, out_doc, out_sc, out_n
+
+    def search_phrase_batch(self, top_docs, term_ords_per_segment, offsets=None, slop=None, scoring=True):
+        """Phrase queries over every segment: term_ords_per_segment[s] [n_queries, n_terms] in segment s's ordinals, in offset
+        order, ABSENT_TERM where segment s does not hold the term (it then matches nothing there), NO_TERM pads.  The weight
+        is Bm25Weight::for_terms over the searcher-wide doc_freq / total_num_docs / average fieldnorm; the per-segment top
+        lists are merged like search_batch.  Returns (segment_ord [nq,k], docs [nq,k], scores [nq,k], n [nq])."""
+        ords = [np.ascontiguousarray(o, np.uint32) for o in term_ords_per_segment]
+        nq, nt = ords[0].shape
+        df = np.zeros((nq, nt), np.int64)
+        for seg, o in zip(self.segments, ords):
+            held = o < seg.n_terms
+            df += np.where(held, seg.doc_freq[np.minimum(o, max(seg.n_terms - 1, 0))].astype(np.int64), 0)
+        real = ords[0] != NO_TERM
+        weights = None
+        if scoring:
+            weights = np.array([Bm25Weight.for_terms(df[q][real[q]], self.total_num_docs, self.average_fieldnorm).weight
+                                for q in range(nq)], np.float32)
+        inner = TopDocs(top_docs.limit + top_docs.offset)
+        parts = []
+        for s_ord, (seg, o) in enumerate(zip(self.segments, ords)):
+            d, sc, n = inner.search_phrase_batch(seg, o, offsets, slop, scoring, weights=weights, average_fieldnorm=self.average_fieldnorm)
+            parts.append((s_ord, d, sc, n))
+        k = top_docs.limit
+        out_seg = np.zeros((nq, k), np.uint32); out_doc = np.zeros((nq, k), np.uint32)
+        out_sc = np.zeros((nq, k), np.float32); out_n = np.zeros(nq, np.uint32)
+        for q in range(nq):
+            segs = np.concatenate([np.full(int(n[q]), s_ord, np.uint32) for s_ord, _, _, n in parts])
+            docs = np.concatenate([d[q, :n[q]] for _, d, _, n in parts])
+            scs = np.concatenate([sc[q, :n[q]] for _, _, sc, n in parts])
+            order = np.lexsort((docs, segs, -scs.astype(np.float64)))[top_docs.offset:top_docs.offset + k]
+            m = order.size
+            out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = segs[order], docs[order], scs[order], m
+        return out_seg, out_doc, out_sc, out_n
+
+
+class PhraseQuery:
+    """tantivy PhraseQuery (phrase_query.rs): terms with position offsets (default 0, 1, 2, ...), sorted stably by offset
+    like new_with_offset_and_slop, and a slop (0: the terms must be adjacent)."""
+
+    def __init__(self, terms, offsets=None, slop=0):
+        terms = [int(t) for t in terms]
+        assert len(terms) > 1, "A phrase query is required to have strictly more than one term."
+        offsets = list(range(len(terms))) if offsets is None else [int(o) for o in offsets]
+        assert len(offsets) == len(terms)
+        pairs = sorted(zip(offsets, terms), key=lambda p: p[0])
+        self.phrase_terms = pairs
+        self.slop = int(slop)
+
+    @staticmethod
+    def rows(queries, n_terms=None):
+        """A list of PhraseQuery -> (term_ords, offsets, slop) arrays for search_phrase_batch (NO_TERM pads)."""
+        nt = n_terms or max(len(q.phrase_terms) for q in queries)
+        t = np.full((len(queries), nt), NO_TERM, np.uint32); o = np.zeros((len(queries), nt), np.uint32)
+        for i, q in enumerate(queries):
+            for j, (off, term) in enumerate(q.phrase_terms):
+                t[i, j], o[i, j] = term, off
+        return t, o, np.array([q.slop for q in queries], np.uint32)
 
 
 class SignalComputer:

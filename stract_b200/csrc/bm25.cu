@@ -77,6 +77,19 @@ struct sb200_segment {
   // sparse result tables go to the host packed (copy_out_tables)
   sb200::DevBuf<uint32_t> p_docs, p_scores; sb200::DevBuf<uint64_t> p_off;
   uint32_t* h_pack = nullptr; size_t h_pack_words = 0;   // page-locked staging: [n counts | offsets (u64) | docs | scores]
+  // positions (sb200_segment_attach_positions, bm25_phrase.cuh)
+  bool has_pos = false;
+  sb200::DevBuf<uint8_t> pos_file;
+  sb200::DevBuf<uint64_t> pos_data_off, pos_tail_off, pos_end_off, pos_count;   // per term
+  sb200::DevBuf<uint32_t> pos_first, pos_nblk;                                   // per term
+  sb200::DevBuf<uint32_t> pos_b_off; sb200::DevBuf<uint8_t> pos_b_w;            // per positions block
+  sb200::DevBuf<uint64_t> pos_base;                                              // per posting block slot
+  std::vector<uint64_t> h_pos_count;
+  // scratch of the phrase path
+  sb200::DevBuf<uint32_t> ph_shift, ph_slop, ph_cdoc, ph_ctf, ph_mcnt, ph_mkey, ph_mdoc, ph_scratch;
+  sb200::DevBuf<float> ph_weight;
+  sb200::DevBuf<uint64_t> ph_coff, ph_pre;
+  sb200::DevBuf<unsigned long long> ph_ov, ph_ovc;
 };
 
 namespace sb200 {
@@ -654,6 +667,7 @@ static int launch_topk_warp(const WParams& P, cudaStream_t s) {
 #include "bm25_or3.cuh"
 #include "bm25_multi.cuh"
 #include "bm25_wand.cuh"
+#include "bm25_phrase.cuh"
 namespace sb200 {
 
 static void seg_view(const sb200_segment* g, SegView& S) {
@@ -1171,6 +1185,183 @@ static int run_batch(sb200_segment* g, const sb200_bm25_batch* b, int mode, cons
   return SB200_OK;
 }
 
+static void pos_view(const sb200_segment* g, PosView& V) {
+  V.f32 = (const uint32_t*)g->pos_file.p; V.data_off = g->pos_data_off.p; V.tail_off = g->pos_tail_off.p; V.end_off = g->pos_end_off.p;
+  V.count = g->pos_count.p; V.first = g->pos_first.p; V.nblk = g->pos_nblk.p; V.b_off = g->pos_b_off.p; V.b_w = g->pos_b_w.p;
+}
+
+// Phrase batch (bm25_phrase.cuh).  Host planning mirrors PhraseWeight::phrase_scorer: a term the segment does not hold empties
+// the phrase; the others are put in Intersection order (stable sort by doc_freq, intersection.rs:69-81) with their shift
+// max_offset - offset.  Queries are processed in groups whose candidate records fit a memory budget.
+static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* docs, float* scores, uint32_t* n_out, sb200_phrase_stats* stats) {
+  NvtxRange nvtx("sb200 phrase top-k batch");
+  cudaStream_t s = g->stream;
+  if (!b || !b->term_ords || !docs || !scores || !n_out) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (b->scoring && (!b->weights || !b->tf_cache256)) SB_FAIL(SB200_EINVAL, "scoring needs weights and tf_cache256");
+  if (g->record != SB200_RECORD_FREQS_POSITIONS) SB_FAIL(SB200_EINVAL, "phrase query on a field without positions (record option %d)", g->record);
+  if (!g->has_pos) SB_FAIL(SB200_EINVAL, "phrase query: no positions attached to the segment (sb200_segment_attach_positions)");
+  const uint32_t nq = b->n_queries, nt = b->n_terms, k = b->k;
+  if (nt < 2 || nt > MAXT) SB_FAIL(SB200_ERANGE, "n_terms %u outside [2,%d]", nt, MAXT);
+  if (k == 0 || k > SB200_MAX_K) SB_FAIL(SB200_ERANGE, "k %u outside [1,%d]", k, SB200_MAX_K);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (nq == 0) return SB200_OK;
+  std::vector<uint32_t> terms((size_t)nq * nt, 0), shift((size_t)nq * nt, 0), nterms(nq, 0), slop(nq, 0);
+  std::vector<float> weight(nq, 0.0f);
+  for (uint32_t q = 0; q < nq; q++) {
+    uint32_t ords[MAXT], offs[MAXT], c = 0;
+    bool absent = false;
+    for (uint32_t t = 0; t < nt; t++) {
+      const uint32_t ord = b->term_ords[(size_t)q * nt + t];
+      if (ord == SB200_NO_TERM) {
+        for (uint32_t u = t; u < nt; u++) if (b->term_ords[(size_t)q * nt + u] != SB200_NO_TERM) SB_FAIL(SB200_EINVAL, "query %u: SB200_NO_TERM pads the end of a row only", q);
+        break;
+      }
+      if (ord == SB200_ABSENT_TERM) absent = true;
+      else if (ord >= g->n_terms) SB_FAIL(SB200_EINVAL, "query %u: term ordinal %u >= %u", q, ord, g->n_terms);
+      ords[c] = ord; offs[c] = b->offsets ? b->offsets[(size_t)q * nt + t] : t; c++;
+    }
+    if (c < 2) SB_FAIL(SB200_EINVAL, "query %u has %u terms: a phrase has 2..%d", q, c, MAXT);
+    slop[q] = b->slop ? b->slop[q] : 0u;
+    weight[q] = b->scoring ? b->weights[q] : 0.0f;
+    if (absent) continue;
+    uint32_t max_off = 0, idx[MAXT];
+    for (uint32_t i = 0; i < c; i++) { max_off = std::max(max_off, offs[i]); idx[i] = i; }
+    std::stable_sort(idx, idx + c, [&](uint32_t x, uint32_t y) { return g->h_df[ords[x]] < g->h_df[ords[y]]; });
+    for (uint32_t i = 0; i < c; i++) { terms[(size_t)q * nt + i] = ords[idx[i]]; shift[(size_t)q * nt + i] = max_off - offs[idx[i]]; }
+    nterms[q] = c;
+  }
+  SB_TRY(ensure(g->q_terms, (size_t)nq * nt)); SB_TRY(ensure(g->ph_shift, (size_t)nq * nt)); SB_TRY(ensure(g->q_nterms, nq));
+  SB_TRY(ensure(g->ph_slop, nq)); SB_TRY(ensure(g->ph_weight, nq)); SB_TRY(ensure(g->q_weights, (size_t)nq * nt)); SB_TRY(ensure(g->q_cache, 256));
+  SB_TRY(ensure(g->o_docs, (size_t)nq * k)); SB_TRY(ensure(g->o_scores, (size_t)nq * k)); SB_TRY(ensure(g->o_n, nq));
+  SB_TRY(ensure(g->counters, 8)); SB_TRY(ensure(g->a3_off, nq)); SB_TRY(ensure(g->a3_cnt, nq)); SB_TRY(ensure(g->ph_mcnt, nq));
+  SB_TRY(ensure(g->ph_ovc, 4)); SB_TRY(ensure(g->ph_pre, (size_t)nq + 1));
+  SB_CUDA(cudaEventRecord(g->ev0, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_terms.p, terms.data(), terms.size() * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->ph_shift.p, shift.data(), shift.size() * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, nterms.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->ph_slop.p, slop.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->ph_weight.p, weight.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemsetAsync(g->q_weights.p, 0, (size_t)nq * nt * 4, s));
+  if (b->scoring) SB_CUDA(cudaMemcpyAsync(g->q_cache.p, b->tf_cache256, 256 * 4, cudaMemcpyDefault, s));
+  else SB_CUDA(cudaMemsetAsync(g->q_cache.p, 0, 256 * 4, s));
+  SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 8 * sizeof(unsigned long long), s));
+  SB_CUDA(cudaMemsetAsync(g->a3_cnt.p, 0, (size_t)nq * 4, s));
+  SB_CUDA(cudaMemsetAsync(g->ph_mcnt.p, 0, (size_t)nq * 4, s));
+  static size_t sel_conf = 0;
+  const size_t sel_smem = (size_t)A3_SEL_CAP * 8;
+  if (sel_conf < sel_smem) { SB_CUDA(cudaFuncSetAttribute(k_and3_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem)); sel_conf = sel_smem; }
+  const size_t cand_smem = (size_t)A3_WARPS * nt * 128 * 12;
+  static size_t cand_conf = 0;
+  if (cand_conf < cand_smem) { SB_CUDA(cudaFuncSetAttribute(k_phrase_cand, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand_smem)); cand_conf = cand_smem; }
+  int n_sm = 132;
+  { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 132; }
+  // candidate records: doc + nt x (u64 offset, u32 tf) + a match (key, doc) per entry
+  uint64_t budget = (uint64_t)2 << 30;
+  if (const char* e = getenv("SB200_PHRASE_BUDGET_MB")) { const long mb = atol(e); if (mb > 0) budget = (uint64_t)mb << 20; }
+  const uint64_t max_entries = std::max<uint64_t>(budget / (12 + 12 * (uint64_t)nt), 1);
+  std::vector<uint64_t> off(nq, 0), pre(nq + 1, 0);
+  std::vector<uint32_t> cnt(nq, 0);
+  std::vector<AUnit> units;
+  // kernel_ms: the device time of the launches alone (the count read-backs between passes are left out)
+  float kms = 0.0f;
+  auto timed = [&](auto&& launch) -> int {
+    SB_CUDA(cudaEventRecord(g->evk0, s));
+    SB_TRY(launch());
+    SB_CUDA(cudaEventRecord(g->evk1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+    return SB200_OK;
+  };
+  uint32_t g0 = 0;
+  while (g0 < nq) {
+    uint64_t entries = 0; uint32_t g1 = g0;
+    units.clear();
+    while (g1 < nq) {
+      const uint32_t dfA = nterms[g1] ? g->h_df[terms[(size_t)g1 * nt]] : 0u;
+      if (g1 > g0 && entries + dfA > max_entries) break;
+      off[g1] = entries; entries += dfA;
+      const uint32_t nblk = (dfA >> 7) + ((dfA & 127u) ? 1u : 0u);
+      for (uint32_t b0 = 0; b0 < nblk; b0 += A3_UNIT_BLOCKS) { AUnit u; u.q = g1; u.blk_lo = b0; u.blk_hi = std::min(nblk, b0 + A3_UNIT_BLOCKS); u._pad = 0; units.push_back(u); }
+      g1++;
+    }
+    const uint32_t n_units = (uint32_t)units.size();
+    const size_t ne = (size_t)std::max<uint64_t>(entries, 1);
+    SB_TRY(ensure(g->ph_cdoc, ne)); SB_TRY(ensure(g->ph_coff, ne * nt)); SB_TRY(ensure(g->ph_ctf, ne * nt));
+    SB_TRY(ensure(g->ph_mkey, ne)); SB_TRY(ensure(g->ph_mdoc, ne)); SB_TRY(ensure(g->a3_units, std::max<size_t>(n_units, 1)));
+    SB_CUDA(cudaMemcpyAsync(g->a3_off.p + g0, off.data() + g0, (size_t)(g1 - g0) * 8, cudaMemcpyHostToDevice, s));
+    if (n_units) {
+      SB_CUDA(cudaMemcpyAsync(g->a3_units.p, units.data(), (size_t)n_units * sizeof(AUnit), cudaMemcpyHostToDevice, s));
+      PhCandParams C;
+      memset(&C, 0, sizeof(C));
+      seg_view(g, C.A.S); C.A.a128 = g->a_post.p; C.A.t_aoff = g->t_aoff.p;
+      C.A.q_terms = g->q_terms.p; C.A.q_nterms = g->q_nterms.p; C.A.q_weights = g->q_weights.p; C.A.cache = g->q_cache.p; C.A.n_terms_max = nt;
+      C.A.units = (const AUnit*)g->a3_units.p; C.A.n_units = n_units;
+      C.A.cand_off = g->a3_off.p; C.A.cand_cnt = g->a3_cnt.p; C.A.counters = g->counters.p;
+      C.pos_base = g->pos_base.p; C.nt = nt; C.c_doc = g->ph_cdoc.p; C.c_off = g->ph_coff.p; C.c_tf = g->ph_ctf.p;
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_cand, div_up(n_units, A3_WARPS), A3_WARPS * 32, cand_smem, s, C); SB_CHECK_LAUNCH(); return SB200_OK; }));
+    }
+    // candidate counts -> the group's prefix (k_phrase_verify maps a candidate to its query by a binary search in it)
+    SB_CUDA(cudaMemcpyAsync(cnt.data() + g0, g->a3_cnt.p + g0, (size_t)(g1 - g0) * 4, cudaMemcpyDeviceToHost, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    const uint32_t ns = g1 - g0;
+    pre[0] = 0;
+    for (uint32_t i = 0; i < ns; i++) pre[i + 1] = pre[i] + cnt[g0 + i];
+    const uint64_t total = pre[ns];
+    if (total) {
+      SB_CUDA(cudaMemcpyAsync(g->ph_pre.p, pre.data(), (size_t)(ns + 1) * 8, cudaMemcpyHostToDevice, s));
+      SB_TRY(ensure(g->ph_ov, 2 * (size_t)total));
+      PhParams V;
+      memset(&V, 0, sizeof(V));
+      pos_view(g, V.V);
+      V.fieldnorm = g->fieldnorm.p; V.cache = g->q_cache.p;
+      V.q_terms = g->q_terms.p; V.q_shift = g->ph_shift.p; V.q_nterms = g->q_nterms.p; V.q_slop = g->ph_slop.p; V.q_weight = g->ph_weight.p;
+      V.nt = nt; V.scoring = b->scoring ? 1 : 0;
+      V.cand_off = g->a3_off.p; V.cand_pre = g->ph_pre.p; V.slot0 = g0; V.n_slots = ns;
+      V.c_doc = g->ph_cdoc.p; V.c_off = g->ph_coff.p; V.c_tf = g->ph_ctf.p;
+      V.m_cnt = g->ph_mcnt.p; V.m_key = g->ph_mkey.p; V.m_doc = g->ph_mdoc.p; V.counters = g->counters.p;
+      unsigned long long* lists[2] = {(unsigned long long*)g->ph_ov.p, (unsigned long long*)g->ph_ov.p + total};
+      V.list = nullptr; V.n = total; V.factor = 1; V.ov_list = lists[0]; V.ov = g->ph_ovc.p; V.scratch_cursor = g->ph_ovc.p + 2;
+      SB_CUDA(cudaMemsetAsync(g->ph_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+      const unsigned grid = (unsigned)std::min<uint64_t>(div_up(total, PH_WARPS), (uint64_t)n_sm * 16);
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_verify, grid, PH_WARPS * 32, 0, s, V); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      // candidates whose lists do not fit shared memory, then those whose carrying-slop merge outgrew its buffers
+      uint64_t factor = 1;
+      for (int pass = 0;; pass++) {
+        unsigned long long ov[4] = {0, 0, 0, 0};
+        SB_CUDA(cudaMemcpyAsync(ov, g->ph_ovc.p, sizeof(ov), cudaMemcpyDeviceToHost, s));
+        SB_CUDA(cudaStreamSynchronize(s));
+        if (ov[0] == 0) break;
+        if (pass >= 8) SB_FAIL(SB200_ENOMEM, "phrase verification: the carrying-slop buffers of %llu candidates still overflow", ov[0]);
+        factor = std::max<uint64_t>(factor * 4, ov[3]);   // 4x, or the merge length the overflowing candidates asked for
+        if (factor > 0xFFFFFFFFull) SB_FAIL(SB200_ENOMEM, "phrase verification: carrying-slop buffers beyond 2^32 entries");
+        SB_TRY(ensure(g->ph_scratch, (size_t)(ov[1] * (1 + 4ull * factor) + 64)));
+        V.list = lists[pass & 1]; V.n = ov[0]; V.ov_list = lists[(pass + 1) & 1];
+        V.scratch = g->ph_scratch.p; V.factor = (uint32_t)factor;
+        SB_CUDA(cudaMemsetAsync(g->ph_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+        const unsigned grid2 = (unsigned)std::min<uint64_t>(div_up(ov[0], PH_WARPS), (uint64_t)n_sm * 16);
+        SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_verify, grid2, PH_WARPS * 32, 0, s, V); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      }
+    }
+    SB_TRY(timed([&]() -> int {
+      SB_LAUNCH(k_and3_select, ns, 256, sel_smem, s, g->a3_off.p, g->ph_mcnt.p, g->ph_mkey.p, g->ph_mdoc.p, (const uint32_t*)nullptr, g0, k,
+                g->o_docs.p, g->o_scores.p, g->o_n.p);
+      SB_CHECK_LAUNCH(); return SB200_OK; }));
+    g0 = g1;
+  }
+  SB_TRY(copy_out_tables(g, nq, k, docs, scores, nullptr, n_out));
+  unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  SB_CUDA(cudaEventRecord(g->ev1, s));
+  SB_CUDA(cudaStreamSynchronize(s));
+  if (h[2]) SB_FAIL(SB200_EFORMAT, "%llu phrase work items met inconsistent posting / position data", h[2]);
+  if (h[5]) SB_FAIL(SB200_ENOMEM, "phrase verification: %llu candidates need carrying-slop buffers beyond 2^32 entries", h[5]);
+  if (stats) {
+    stats->candidates = h[0]; stats->matches = h[1]; stats->positions_decoded = h[3]; stats->position_bytes = h[4];
+    cudaEventElapsedTime(&stats->ms, g->ev0, g->ev1); stats->kernel_ms = kms;
+  }
+  return SB200_OK;
+}
+
 }  // namespace sb200
 using namespace sb200;
 
@@ -1214,6 +1405,30 @@ __global__ void k_term_info_store(const uint8_t* __restrict__ file, uint64_t len
   }
   out[ord] = ti;
 }
+// TermInfo.positions_range of every ordinal (term_info_store.rs:63-91): the block's reference range sits after its postings
+// range in the TermInfoBlockMeta (TermInfo::serialize, term_info.rs:41-47), the bit-packed start follows the postings start
+__global__ void k_term_info_store_positions(const uint8_t* __restrict__ file, uint64_t len, uint64_t meta_len, uint64_t n_terms,
+                                            uint64_t* pos_off, uint64_t* pos_len, int* err) {
+  const uint64_t ord = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (ord >= n_terms) return;
+  const uint8_t* m = file + 16 + (ord >> 8) * 47;
+  const uint8_t* infos = file + 16 + meta_len;
+  const uint64_t infos_len = len - 16 - meta_len;
+  const uint64_t off = tis_u64(m, 8);
+  const uint64_t rqs = tis_u64(m + 28, 8), rql = tis_u64(m + 36, 8);
+  const uint32_t dfb = m[44], pb = m[45], qb = m[46];
+  const uint32_t inner = (uint32_t)(ord & 255u);
+  uint64_t s = rqs, l = rql;
+  if (inner != 0) {
+    if (off > infos_len || dfb > 56 || pb > 56 || qb > 56) { *err = 1; return; }
+    const uint64_t nb = (uint64_t)dfb + pb + qb, a0 = nb * (inner - 1) + pb;
+    const uint8_t* d = infos + off; const uint64_t dl = infos_len - off;
+    const uint64_t qs = rqs + tis_bits(d, dl, a0, qb), qe = rqs + tis_bits(d, dl, a0 + nb, qb);
+    if (qe < qs) { *err = 2; return; }
+    s = qs; l = qe - qs;
+  }
+  pos_off[ord] = s; pos_len[ord] = l;
+}
 }  // namespace sb200
 
 extern "C" {
@@ -1242,6 +1457,34 @@ int sb200_term_info_store_decode(const uint8_t* store, uint64_t len, int device,
   SB_CUDA(cudaMemcpy(&h_err, d_err.p, sizeof(int), cudaMemcpyDeviceToHost));
   if (h_err) SB_FAIL(SB200_EFORMAT, "term info store is inconsistent (code %d)", h_err);
   SB_CUDA(cudaMemcpy(infos, d_out.p, k * sizeof(sb200_term_info), cudaMemcpyDefault));
+  return SB200_OK;
+}
+
+int sb200_term_info_store_decode_positions(const uint8_t* store, uint64_t len, int device, uint64_t* positions_off, uint64_t* positions_len,
+                                           uint64_t cap, uint64_t* n_terms) {
+  using namespace sb200;
+  if (!store || !n_terms) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (len < 16) SB_FAIL(SB200_EFORMAT, "term info store shorter than its 16-byte header");
+  SB_CUDA(cudaSetDevice(device));
+  uint8_t head[16];
+  SB_CUDA(cudaMemcpy(head, store, 16, cudaMemcpyDefault));
+  uint64_t meta_len = 0, n = 0;
+  memcpy(&meta_len, head, 8); memcpy(&n, head + 8, 8);
+  if (meta_len > len - 16 || meta_len != 47ull * ((n + 255) / 256)) SB_FAIL(SB200_EFORMAT, "term info store: %llu terms need %llu bytes of block metadata, header says %llu", (unsigned long long)n, (unsigned long long)(47ull * ((n + 255) / 256)), (unsigned long long)meta_len);
+  *n_terms = n;
+  const uint64_t k = std::min<uint64_t>(n, cap);
+  if (!positions_off || !positions_len || k == 0) return SB200_OK;
+  DevBuf<uint8_t> d_store; DevBuf<uint64_t> d_off, d_len; DevBuf<int> d_err;
+  SB_TRY(d_store.alloc(len)); SB_TRY(d_off.alloc(n)); SB_TRY(d_len.alloc(n)); SB_TRY(d_err.alloc(1));
+  SB_CUDA(cudaMemcpy(d_store.p, store, len, cudaMemcpyDefault));
+  SB_CUDA(cudaMemset(d_err.p, 0, sizeof(int)));
+  SB_LAUNCH(k_term_info_store_positions, div_up(n, 256), 256, 0, (cudaStream_t)0, d_store.p, len, meta_len, n, d_off.p, d_len.p, d_err.p);
+  SB_CHECK_LAUNCH();
+  int h_err = 0;
+  SB_CUDA(cudaMemcpy(&h_err, d_err.p, sizeof(int), cudaMemcpyDeviceToHost));
+  if (h_err) SB_FAIL(SB200_EFORMAT, "term info store is inconsistent (code %d)", h_err);
+  SB_CUDA(cudaMemcpy(positions_off, d_off.p, k * 8, cudaMemcpyDefault));
+  SB_CUDA(cudaMemcpy(positions_len, d_len.p, k * 8, cudaMemcpyDefault));
   return SB200_OK;
 }
 
@@ -1353,6 +1596,9 @@ int sb200_segment_get_info(const sb200_segment* g, sb200_segment_info* info) {
   info->n_terms = g->n_terms; info->n_blocks = g->n_blocks; info->n_postings = g->n_postings; info->max_doc = g->max_doc; info->_pad = 0;
   info->hbm_bytes = g->postings.bytes() + g->fieldnorm.bytes() + g->t_first.bytes() + g->t_data_off.bytes() + g->t_end_off.bytes() +
                     g->t_df.bytes() + g->b_last.bytes() + g->b_off.bytes() + g->b_bits.bytes() + g->b_bw.bytes();
+  if (g->has_pos)
+    info->hbm_bytes += g->pos_file.bytes() + g->pos_data_off.bytes() + g->pos_tail_off.bytes() + g->pos_end_off.bytes() + g->pos_count.bytes() +
+                       g->pos_first.bytes() + g->pos_nblk.bytes() + g->pos_b_off.bytes() + g->pos_b_w.bytes() + g->pos_base.bytes();
   info->stage_ms = g->stage_ms;
   return SB200_OK;
 }
@@ -1478,6 +1724,93 @@ int sb200_bm25_topk(sb200_segment* seg, const uint32_t* term_ords, const float* 
   sb200_bm25_batch b;
   b.n_queries = 1; b.n_terms = n_terms; b.term_ords = term_ords; b.weights = weights; b.tf_cache256 = tf_cache256; b.mode = mode; b.k = k;
   return sb200_bm25_topk_batch(seg, &b, docs, scores, n_out, nullptr);
+}
+
+int sb200_segment_attach_positions(sb200_segment* g, const uint8_t* positions_file, uint64_t len, const uint64_t* positions_off,
+                                   const uint64_t* positions_len) {
+  if (!g) SB_FAIL(SB200_EINVAL, "NULL segment handle");
+  if (g->record != SB200_RECORD_FREQS_POSITIONS)
+    SB_FAIL(SB200_EINVAL, "the segment was opened with record option %d: positions need WithFreqsAndPositions (2)", g->record);
+  const uint32_t n = g->n_terms;
+  if ((len && !positions_file) || (n && (!positions_off || !positions_len))) SB_FAIL(SB200_EINVAL, "NULL argument");
+  SB_CUDA(cudaSetDevice(g->device));
+  g->has_pos = false;
+  cudaStream_t s = g->stream;
+  std::vector<uint64_t> ho(n), hl(n);
+  SB_CUDA(cudaMemcpy(ho.data(), positions_off, (size_t)n * 8, cudaMemcpyDefault));
+  SB_CUDA(cudaMemcpy(hl.data(), positions_len, (size_t)n * 8, cudaMemcpyDefault));
+  for (uint32_t t = 0; t < n; t++)
+    if (ho[t] > len || hl[t] > len - ho[t] || hl[t] == 0) SB_FAIL(SB200_EFORMAT, "term %u: positions range [%llu, +%llu) outside the %llu-byte file or empty", t,
+                                                                 (unsigned long long)ho[t], (unsigned long long)hl[t], (unsigned long long)len);
+  SB_TRY(g->pos_file.alloc(len + 64));
+  SB_CUDA(cudaMemsetAsync(g->pos_file.p + len, 0, 64, s));
+  SB_TRY(copy_in(g->pos_file.p, positions_file, len, s));
+  DevBuf<uint64_t> d_off, d_len, d_hdr; DevBuf<int> d_err;
+  SB_TRY(d_off.alloc(n + 1)); SB_TRY(d_len.alloc(n + 1)); SB_TRY(d_hdr.alloc(n + 1)); SB_TRY(d_err.alloc(1));
+  SB_TRY(g->pos_nblk.alloc(n + 1)); SB_TRY(g->pos_first.alloc(n + 1));
+  SB_CUDA(cudaMemcpyAsync(d_off.p, ho.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(d_len.p, hl.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemsetAsync(d_err.p, 0, sizeof(int), s));
+  std::vector<uint32_t> nblk(n + 1, 0), first(n + 1, 0);
+  if (n) {
+    SB_LAUNCH(k_pos_header, div_up(n, 256), 256, 0, s, g->pos_file.p, d_off.p, d_len.p, n, g->pos_nblk.p, d_hdr.p, d_err.p);
+    SB_CHECK_LAUNCH();
+    SB_CUDA(cudaMemcpyAsync(nblk.data(), g->pos_nblk.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  }
+  int h_err = 0;
+  SB_CUDA(cudaMemcpyAsync(&h_err, d_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  SB_CUDA(cudaStreamSynchronize(s));
+  if (h_err) SB_FAIL(SB200_EFORMAT, "malformed positions: a term's VInt block count is unterminated or exceeds its range");
+  uint64_t blocks = 0;
+  for (uint32_t t = 0; t < n; t++) {
+    first[t] = (uint32_t)blocks; blocks += nblk[t];
+    if (blocks >= 0xFFFFFFF0ull) SB_FAIL(SB200_ERANGE, "more than 2^32 positions blocks");
+  }
+  first[n] = (uint32_t)blocks;
+  const uint64_t slots = g->n_blocks + n;   // posting block slots: n_full + 1 per term
+  SB_TRY(g->pos_b_off.alloc(blocks + 1)); SB_TRY(g->pos_b_w.alloc(blocks + 1));
+  SB_TRY(g->pos_data_off.alloc(n + 1)); SB_TRY(g->pos_tail_off.alloc(n + 1)); SB_TRY(g->pos_end_off.alloc(n + 1)); SB_TRY(g->pos_count.alloc(n + 1));
+  SB_TRY(g->pos_base.alloc(slots + 1));
+  SB_CUDA(cudaMemcpyAsync(g->pos_first.p, first.data(), (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, s));
+  g->h_pos_count.assign(n, 0);
+  if (n) {
+    SB_LAUNCH(k_pos_dir, div_up((uint64_t)n * 32, 256), 256, 0, s, g->pos_file.p, d_off.p, d_len.p, d_hdr.p, g->pos_nblk.p, g->pos_first.p, n,
+              g->postings.p, g->t_data_off.p, g->t_df.p, g->t_first.p, g->pos_data_off.p, g->pos_tail_off.p, g->pos_end_off.p, g->pos_count.p,
+              g->pos_b_off.p, g->pos_b_w.p, g->pos_base.p, d_err.p);
+    SB_CHECK_LAUNCH();
+    SB_CUDA(cudaMemcpyAsync(g->h_pos_count.data(), g->pos_count.p, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+  }
+  SB_CUDA(cudaMemcpyAsync(&h_err, d_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  SB_CUDA(cudaStreamSynchronize(s));
+  if (h_err) SB_FAIL(SB200_EFORMAT, "malformed positions: bit width > 32, blocks beyond the term's range, or a tail that is not a run of < 128 VInts");
+  g->has_pos = true;
+  return SB200_OK;
+}
+
+int sb200_positions_read(sb200_segment* g, uint32_t term, uint64_t offset, uint32_t n, uint32_t* out) {
+  if (!g || (n && !out)) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (!g->has_pos) SB_FAIL(SB200_EINVAL, "no positions attached to the segment");
+  if (term >= g->n_terms) SB_FAIL(SB200_EINVAL, "term ordinal %u >= %u", term, g->n_terms);
+  if (offset > g->h_pos_count[term] || n > g->h_pos_count[term] - offset)
+    SB_FAIL(SB200_ERANGE, "positions [%llu, +%u) of term %u: it has %llu", (unsigned long long)offset, n, term, (unsigned long long)g->h_pos_count[term]);
+  if (n == 0) return SB200_OK;
+  SB_CUDA(cudaSetDevice(g->device));
+  DevBuf<uint32_t> tmp;
+  uint32_t* dst = out;
+  if (!is_device_ptr(out)) { SB_TRY(tmp.alloc(n)); dst = tmp.p; }
+  PosView V; pos_view(g, V);
+  SB_LAUNCH(k_positions_read, 1, 32, 0, g->stream, V, term, offset, n, dst);
+  SB_CHECK_LAUNCH();
+  if (dst != out) SB_CUDA(cudaMemcpyAsync(out, dst, (size_t)n * 4, cudaMemcpyDeviceToHost, g->stream));
+  SB_CUDA(cudaStreamSynchronize(g->stream));
+  return SB200_OK;
+}
+
+int sb200_phrase_topk_batch(sb200_segment* seg, const sb200_phrase_batch* batch, uint32_t* docs, float* scores, uint32_t* n_out,
+                            sb200_phrase_stats* stats) {
+  if (!seg) SB_FAIL(SB200_EINVAL, "NULL segment handle");
+  SB_CUDA(cudaSetDevice(seg->device));
+  return run_phrase(seg, batch, docs, scores, n_out, stats);
 }
 
 int sb200_multi_signal_topk_batch(const sb200_multi_signal_batch* batch, uint32_t* docs, double* totals, uint32_t* n_out,

@@ -185,4 +185,55 @@ int sb200_postings_encode_ex(const uint32_t* docs, const uint32_t* tfs, const ui
   return SB200_OK;
 }
 
+// PositionSerializer (tantivy/src/positions/serializer.rs:47-87): per term [VInt n_blocks][bit width per block][blocks][vint
+// tail]; a block is 128 deltas packed with BitPacker4x::compress (compress_block_unsorted: the width of their OR), the tail
+// is compress_vint_unsorted.  Deltas restart at every posting (the first one is the position itself).
+int sb200_positions_encode(const uint32_t* positions, const uint32_t* tfs, const uint64_t* term_off, uint32_t n_terms,
+                           uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* positions_off, uint64_t* positions_len) {
+  using namespace sb200;
+  if (!term_off || !out_len) SB_FAIL(SB200_EINVAL, "NULL argument");
+  const uint64_t n_post = n_terms ? term_off[n_terms] : 0;
+  if (n_post && !tfs) SB_FAIL(SB200_EINVAL, "tfs is NULL");
+  uint64_t n_pos = 0;
+  for (uint32_t t = 0; t < n_terms; t++)
+    if (term_off[t + 1] < term_off[t]) SB_FAIL(SB200_EINVAL, "term_off must be non-decreasing");
+  for (uint64_t p = 0; p < n_post; p++) n_pos += tfs[p];
+  if (n_pos && !positions) SB_FAIL(SB200_EINVAL, "positions is NULL");
+  std::vector<uint8_t> buf, bits, body;
+  uint64_t at_pos = 0;
+  uint32_t block[128];
+  for (uint32_t t = 0; t < n_terms; t++) {
+    bits.clear(); body.clear();
+    uint32_t fill = 0;
+    for (uint64_t p = term_off[t]; p < term_off[t + 1]; p++) {
+      uint32_t prev = 0;
+      for (uint32_t i = 0; i < tfs[p]; i++) {
+        const uint32_t x = positions[at_pos++];
+        block[fill++] = x - prev;
+        prev = x;
+        if (fill == 128) {
+          uint32_t orred = 0;
+          for (int j = 0; j < 128; j++) orred |= block[j];
+          const int w = width_of(orred);
+          bits.push_back((uint8_t)w);
+          pack4x(block, w, body);
+          fill = 0;
+        }
+      }
+    }
+    for (uint32_t j = 0; j < fill; j++) put_vint(body, block[j]);
+    const uint64_t start = buf.size();
+    put_vint(buf, bits.size());
+    buf.insert(buf.end(), bits.begin(), bits.end());
+    buf.insert(buf.end(), body.begin(), body.end());
+    if (positions_off) positions_off[t] = start;
+    if (positions_len) positions_len[t] = buf.size() - start;
+  }
+  *out_len = buf.size();
+  if (!out) return SB200_OK;
+  if (out_cap < buf.size()) SB_FAIL(SB200_EINVAL, "output buffer too small: need %llu bytes", (unsigned long long)buf.size());
+  memcpy(out, buf.data(), buf.size());
+  return SB200_OK;
+}
+
 }  // extern "C"
