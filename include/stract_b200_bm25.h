@@ -123,7 +123,8 @@ typedef struct {
 } sb200_bm25_batch;
 
 /* ms: device time of the whole call on the handle's stream (query H2D + kernel + result D2H);
- * kernel_ms: the k_topk launch alone (CUDA events around it). */
+ * kernel_ms: the top-k kernels alone, from the first launch to the end of the last (the doc-range merge included),
+ * CUDA events around them. */
 typedef struct { uint64_t postings_scored; uint64_t docs_scored; uint64_t blocks_decoded; float ms; float kernel_ms; } sb200_bm25_stats;
 
 /* Path A.  Outputs are host (or device) arrays: docs/scores [n_queries*k] in rank order (score desc, doc asc),

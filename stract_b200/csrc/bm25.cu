@@ -7,19 +7,24 @@
 //              bit widths u16}; per term {data offset, end offset, doc_freq, first block slot}
 //   signals    optional row-major [max_doc][n_cols] f64 numeric signal scores (one 32-B sector per doc at 4 cols)
 //
-// Kernel k_topk<MODE>: one CTA (128 threads) per query, exhaustive scoring, exact top-k.
-//   The CTA walks all query terms' posting lists block-synchronously: every term keeps one decoded 128-doc
-//   block in shared memory (BitPacker4x unpack: thread k extracts value k from its lane stream, block-wide
-//   prefix sum of the strict deltas).  Each round takes `bound` = the smallest last-doc among the current
-//   blocks; every posting with doc <= bound is final (no later block of any term can contain such a doc),
-//   so membership of a doc in the other terms is a 7-step binary search in their current block.  The term
-//   with the lowest slot that contains the doc "owns" it and computes the score in the reference's f32/f64
-//   operation order; no sort or merge of the lists is needed.  Candidates are pushed (smem atomics) into a
-//   2k-entry buffer with a running threshold exactly like TopNComputer (top_score_collector.rs:501-554);
-//   when it fills, a bitonic sort keeps the best k.  Keys are (order-preserving score bits, ~doc) so the
-//   result order is the reference's (score desc, doc asc) total order.
+// Which kernel serves which batch (all exhaustive, exact top-k, scores in the reference's f32/f64 operation order):
+//   AND                  k_and3 + k_and3_select (bm25_and3.cuh): one warp per (query, 4 blocks of its rarest clause)
+//                        appends the hits to a candidate list, the select kernel takes the top-k per query.
+//   OR, signal combine   k_or3<MODE, TMAX> (bm25_or3.cuh): one warp per work item walks the terms' posting lists
+//                        block-synchronously with TMA staging; TMAX is the smallest of 2/3/5/8 covering the batch.
+//   k_topk_warp<MODE> (bm25_warp.cuh), the same walk without k_or3's specialisations, takes the two batches the kernels
+//   above do not:
+//     * AND with a single-clause query above 65 536 postings: every posting of it is a hit, so k_and3's candidate
+//       list would be the whole posting list and the select pass would crawl through it;
+//     * signal combine with max_docs: k_or3 has no max_docs short circuit.
+//   Block-WAND replay    k_wand (bm25_wand.cuh), one warp per query in the reference's pruning and summation order.
+//   multi-field signals  k_sig_multi<TMAX> (bm25_multi.cuh).
+//   phrases              k_phrase_cand + k_phrase_verify + k_and3_select (bm25_phrase.cuh).
+// A query of the walk kernels much larger than the batch average is cut into doc-range work items (plan_items);
+// k_merge_topk merges their partial top-k lists.  Keys are (order-preserving score bits, ~doc), so the result order
+// is the reference's (score desc, doc asc) total order.
 // Roofline: HBM by bytes (posting bytes + 1 B fieldnorm (+ 8 B x n_cols signals) per scored doc), but at the
-// configured sizes the postings file is L2-resident and the kernel is bound by unpack/search issue rate.
+// configured sizes the postings file is L2-resident and the kernels are bound by unpack/search issue rate.
 #include "common.cuh"
 #include "../../include/stract_b200_bm25.h"
 
@@ -160,135 +165,6 @@ __device__ __forceinline__ float unord_f32(uint32_t o) { return __uint_as_float(
 __device__ __forceinline__ uint64_t ord_f64(double f) { const uint64_t b = (uint64_t)__double_as_longlong(f); return (b >> 63) ? ~b : (b | 0x8000000000000000ull); }
 __device__ __forceinline__ double unord_f64(uint64_t o) { return __longlong_as_double((long long)((o >> 63) ? (o & 0x7FFFFFFFFFFFFFFFull) : ~o)); }
 
-struct TermState {
-  uint64_t data_off, end_off;
-  uint32_t first, nfull, df, cur_blk, len, pos, last_doc, prev_last, done, tail_done;
-  float weight;
-};
-
-struct Smem {
-  uint32_t* docs; uint32_t* tfs;    // [MAXT][128]
-  uint32_t* stage;                   // 336 words: one packed block (<= 1024 B) or the vint tail (<= 1280 B)
-  uint32_t* vals;                    // 256 tail values
-  float* cache;                      // 256
-  TermState* st;                     // [MAXT]
-  uint64_t* khi; uint32_t* klo;      // [CAP]
-  uint32_t* misc;                    // [32] scratch: warp totals, counters
-};
-
-__device__ __forceinline__ uint32_t extract_bits(const uint32_t* words, uint32_t nb, uint32_t k) {
-  if (nb == 0) return 0;
-  const uint32_t lane4 = k & 3u, slot = k >> 2, bit = slot * nb, w = bit >> 5, sh = bit & 31u;
-  const uint32_t lo = words[w * 4 + lane4];
-  const uint32_t hi = (sh + nb > 32) ? words[(w + 1) * 4 + lane4] : 0u;
-  const uint32_t v = __funnelshift_r(lo, hi, sh);
-  return nb == 32 ? v : (v & ((1u << nb) - 1u));
-}
-
-// inclusive scan over the 128 threads of the CTA (wrapping u32); uses misc[0..3]; two barriers
-__device__ __forceinline__ uint32_t cta_scan_incl(uint32_t x, uint32_t* misc) {
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t n = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += n; }
-  if (lane == 31) misc[warp] = x;
-  __syncthreads();
-  uint32_t add = 0;
-  for (uint32_t w = 0; w < warp; w++) add += misc[w];
-  __syncthreads();
-  return x + add;
-}
-
-// stage `nbytes` of the postings file starting at absolute byte `gbyte` into aligned shared words
-__device__ __forceinline__ void stage_bytes(const SegView& S, uint64_t gbyte, uint32_t nbytes, uint32_t* stage) {
-  const uint64_t w0 = gbyte >> 2; const uint32_t sh = (uint32_t)(gbyte & 3u) * 8u;
-  const uint32_t nwords = (nbytes + 3) >> 2;
-  for (uint32_t w = threadIdx.x; w < nwords; w += NT) {
-    const uint32_t lo = __ldg(S.p32 + w0 + w), hi = __ldg(S.p32 + w0 + w + 1);
-    stage[w] = __funnelshift_r(lo, hi, sh);
-  }
-}
-
-// decode the next block of term slot s into docs[s]/tfs[s]; every thread of the CTA calls it
-__device__ void decode_next(const SegView& S, Smem& M, int s) {
-  TermState& T = M.st[s];
-  uint32_t* docs = M.docs + s * 128; uint32_t* tfs = M.tfs + s * 128;
-  __syncthreads();
-  const uint32_t blk = T.cur_blk, prev_last = T.prev_last;
-  if (blk < T.nfull) {
-    const uint32_t idx = T.first + blk;
-    const uint32_t bits = S.b_bits[idx], db = bits & 0x3fu, strict = (bits >> 6) & 1u, tb = bits >> 8;
-    stage_bytes(S, T.data_off + S.b_off[idx], (db + tb) * 16u, M.stage);
-    __syncthreads();
-    const uint32_t k = threadIdx.x;
-    const uint32_t delta = extract_bits(M.stage, db, k) + strict;
-    const uint32_t tf = (S.record >= 1) ? extract_bits(M.stage + db * 4, tb, k) + strict : 1u;
-    const uint32_t pre = cta_scan_incl(delta, M.misc);
-    const uint32_t base = (strict && prev_last == 0) ? 0xFFFFFFFFu : prev_last;  // offset 0 == None (compression/mod.rs:36)
-    docs[k] = base + pre; tfs[k] = tf;
-    __syncthreads();
-    if (threadIdx.x == 0) { T.len = 128; T.pos = 0; T.last_doc = docs[127]; T.prev_last = docs[127]; T.cur_blk = blk + 1; }
-  } else {
-    const uint32_t n = T.df - T.nfull * 128u;
-    const uint64_t tail_off = T.data_off + S.b_off[T.first + T.nfull];
-    const uint32_t nbytes = (uint32_t)min((uint64_t)1340, T.end_off - tail_off);
-    stage_bytes(S, tail_off, nbytes, M.stage);
-    for (uint32_t i = threadIdx.x; i < 256; i += NT) M.vals[i] = (i < 128) ? 0u : 1u;
-    __syncthreads();
-    if (threadIdx.x < 32) {  // warp 0: vint values = runs of bytes ending with the stop bit (compression/vint.rs)
-      const uint8_t* bytes = (const uint8_t*)M.stage;
-      const uint32_t lane = threadIdx.x;
-      uint32_t seen = 0;
-      const uint32_t want = (S.record >= 1) ? 2 * n : n;
-      for (uint32_t base = 0; base < nbytes && seen < want; base += 32) {
-        const uint32_t b = base + lane;
-        const bool stop = (b < nbytes) && (bytes[b] & 0x80u);
-        const unsigned m = __ballot_sync(0xffffffffu, stop);
-        if (stop) {
-          const uint32_t idx = seen + __popc(m & ((1u << lane) - 1u));
-          if (idx < want) {
-            uint32_t start = b;
-            while (start > 0 && !(bytes[start - 1] & 0x80u) && b - start < 4) start--;
-            uint32_t v = 0;
-            for (uint32_t i = start; i <= b; i++) v += (uint32_t)(bytes[i] & 0x7Fu) << (7 * (i - start));
-            M.vals[idx < n ? idx : 128 + (idx - n)] = v;
-          }
-        }
-        seen += __popc(m);
-      }
-    }
-    __syncthreads();
-    const uint32_t k = threadIdx.x;
-    const uint32_t pre = cta_scan_incl(k < n ? M.vals[k] : 0u, M.misc);
-    docs[k] = (k < n) ? prev_last + pre : TERMINATED;
-    tfs[k] = (k < n) ? M.vals[128 + k] : 0u;
-    __syncthreads();
-    if (threadIdx.x == 0) { T.len = n; T.pos = 0; T.last_doc = n ? docs[n - 1] : 0; T.prev_last = T.last_doc; T.cur_blk = blk + 1; T.tail_done = 1; }
-  }
-  __syncthreads();
-}
-
-// advance term slot s to the first full block (>= its cursor) whose last doc is >= L; all threads call it
-__device__ void dir_skip(const SegView& S, Smem& M, int s, uint32_t L) {
-  __syncthreads();
-  const TermState& t = M.st[s];
-  const uint32_t first = t.first, nfull = t.nfull, tid = threadIdx.x;
-  uint32_t j = nfull;
-  for (uint32_t base = t.cur_blk; base < nfull; base += NT) {
-    const uint32_t idx = base + tid;
-    const bool pred = idx < nfull && __ldg(S.b_last + first + idx) >= L;
-    const unsigned m = __ballot_sync(0xffffffffu, pred);
-    if ((tid & 31) == 0) M.misc[tid >> 5] = m ? base + (tid & ~31u) + (uint32_t)__ffs(m) - 1u : 0xFFFFFFFFu;
-    __syncthreads();
-    const uint32_t best = min(min(M.misc[0], M.misc[1]), min(M.misc[2], M.misc[3]));
-    __syncthreads();
-    if (best != 0xFFFFFFFFu) { j = best; break; }
-  }
-  if (tid == 0) {
-    TermState& w = M.st[s];
-    if (j > w.cur_blk) { w.cur_blk = j; w.prev_last = S.b_last[first + j - 1]; }
-  }
-  __syncthreads();
-}
-
 // first index in the sorted 128-entry block with value >= x (branchless, block_search.rs:23-34)
 __device__ __forceinline__ uint32_t lower_bound128(const uint32_t* a, uint32_t x) {
   uint32_t start = 0;
@@ -301,280 +177,6 @@ __device__ __forceinline__ uint32_t lower_bound128(const uint32_t* a, uint32_t x
 }
 
 __device__ __forceinline__ bool key_gt(uint64_t ah, uint32_t al, uint64_t bh, uint32_t bl) { return ah > bh || (ah == bh && al > bl); }
-
-// sort the CAP-entry key buffer descending (bitonic), CAP a power of two
-__device__ void sort_keys_desc(Smem& M, uint32_t cap) {
-  for (uint32_t size = 2; size <= cap; size <<= 1) {
-    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      for (uint32_t i = threadIdx.x; i < (cap >> 1); i += NT) {
-        const uint32_t lo = 2 * i - (i & (stride - 1));
-        const uint32_t hi = lo + stride;
-        const bool desc = ((lo & size) == 0);
-        const uint64_t ah = M.khi[lo], bh = M.khi[hi]; const uint32_t al = M.klo[lo], bl = M.klo[hi];
-        const bool swap = desc ? key_gt(bh, bl, ah, al) : key_gt(ah, al, bh, bl);
-        if (swap) { M.khi[lo] = bh; M.klo[lo] = bl; M.khi[hi] = ah; M.klo[hi] = al; }
-      }
-    }
-  }
-  __syncthreads();
-}
-
-struct Params {
-  SegView S;
-  const uint32_t* q_terms; const uint32_t* q_nterms; const float* q_weights; const float* cache;
-  const uint32_t* q_orig;   // slot -> caller's query index (slots are ordered by decreasing work)
-  uint32_t n_terms_max, k, cap;
-  // path B
-  float k1p1; double coeff_text; const double* sig; uint32_t n_cols; const double* coeffs; uint32_t max_docs;
-  // out
-  uint32_t* o_docs; float* o_scores; double* o_totals; uint32_t* o_n; unsigned long long* counters;
-};
-
-// MODE 0: AND (tantivy Intersection order), 1: OR (tantivy weights, query-order sum), 2: Stract signal combine
-template <int MODE>
-__global__ void __launch_bounds__(NT) k_topk(const Params P) {
-  SB_DYN_SMEM(smem_raw);
-  Smem M;
-  {
-    unsigned char* p = smem_raw;
-    M.khi = (uint64_t*)p; p += (size_t)P.cap * 8;
-    M.st = (TermState*)p; p += sizeof(TermState) * MAXT;
-    M.klo = (uint32_t*)p; p += (size_t)P.cap * 4;
-    M.docs = (uint32_t*)p; p += MAXT * 128 * 4;
-    M.tfs = (uint32_t*)p; p += MAXT * 128 * 4;
-    M.stage = (uint32_t*)p; p += 344 * 4;
-    M.vals = (uint32_t*)p; p += 256 * 4;
-    M.cache = (float*)p; p += 256 * 4;
-    M.misc = (uint32_t*)p;
-  }
-  const SegView& S = P.S;
-  const uint32_t q = blockIdx.x;
-  const uint32_t oq = P.q_orig ? P.q_orig[q] : q;
-  const uint32_t T = P.q_nterms[q];
-  const uint32_t tid = threadIdx.x;
-  uint32_t* s_count = M.misc + 8;     // entries in the key buffer
-  uint32_t* s_flag = M.misc + 9;      // threshold valid
-  uint32_t* s_rstart = M.misc + 12;   // [MAXT+1] prefix of the round's per-term entry counts
-  uint32_t* s_rhi = M.misc + 22;      // [MAXT]
-  uint64_t* s_thr_hi = (uint64_t*)(M.misc + 30); uint32_t* s_thr_lo = M.misc + 10;
-  for (uint32_t i = tid; i < 256; i += NT) M.cache[i] = P.cache[i];
-  for (uint32_t i = tid; i < P.cap; i += NT) { M.khi[i] = 0; M.klo[i] = 0; }
-  if (tid < MAXT) {
-    TermState& t = M.st[tid];
-    t.done = 1; t.len = 0; t.pos = 0;
-    if (tid < T) {
-      const uint32_t ord = P.q_terms[(size_t)q * P.n_terms_max + tid];
-      t.data_off = S.t_data_off[ord]; t.end_off = S.t_end_off[ord]; t.first = S.t_first[ord]; t.df = S.t_df[ord];
-      t.nfull = t.df >> 7; t.cur_blk = 0; t.last_doc = 0; t.prev_last = 0; t.tail_done = 0;
-      t.done = (t.df == 0); t.weight = P.q_weights[(size_t)q * P.n_terms_max + tid];
-    }
-  }
-  if (tid == 0) { *s_count = 0; *s_flag = 0; *s_thr_hi = 0; *s_thr_lo = 0; }
-  __syncthreads();
-  unsigned long long my_docs = 0, my_blocks = 0;
-  unsigned bad_doc = 0u;
-  uint32_t cand_seen = 0;  // path B short-circuit counter (uniform)
-  bool stop_all = (T == 0);
-  // watchdog: every pass of the loop below consumes a block, skips blocks or advances a cursor; a corrupt file
-  // must not be able to spin a CTA forever
-  unsigned long long budget = 64;
-  for (uint32_t s = 0; s < T; s++) budget += 132ull * (M.st[s].nfull + 2);
-
-  while (!stop_all) {
-    if (budget-- == 0) { if (tid == 0) atomicAdd(P.counters + 2, 1ull); break; }
-    // (1) refill exhausted blocks.  AND: a match is >= every term's head, so before decoding the next block of a
-    // term we jump over every block whose last doc is below L = max head of the other terms, using the block
-    // directory (the skip-list seek of Intersection::advance, intersection.rs:95-125 / skip.rs:243-254).
-    for (uint32_t s = 0; s < T; s++) {
-      const TermState& t = M.st[s];
-      if (!t.done && t.pos >= t.len) {
-        if (MODE == 0 && T > 1) {
-          uint32_t L = 0;
-          for (uint32_t x = 0; x < T; x++) { const TermState& u = M.st[x]; if (x != s && !u.done && u.pos < u.len) L = max(L, M.docs[x * 128 + u.pos]); }
-          if (L > 0 && t.cur_blk < t.nfull) dir_skip(S, M, s, L);
-        }
-        const bool more = (t.cur_blk < t.nfull) || (t.cur_blk == t.nfull && !t.tail_done && (t.df & 127u));
-        if (more) { decode_next(S, M, s); my_blocks++; }
-        else { __syncthreads(); if (tid == 0) M.st[s].done = 1; __syncthreads(); }
-      }
-    }
-    // (1b) AND: blocks already decoded but entirely below L are dead, and so are the leading docs below L
-    if (MODE == 0 && T > 1) {
-      bool alive = true; uint32_t L = 0;
-      for (uint32_t s = 0; s < T; s++) { const TermState& t = M.st[s]; if (t.done) alive = false; else L = max(L, M.docs[s * 128 + t.pos]); }
-      if (alive) {
-        bool dead = false;
-        for (uint32_t s = 0; s < T; s++) if (M.st[s].last_doc < L) dead = true;
-        __syncthreads();
-        if (tid < T) {
-          TermState& w = M.st[tid];
-          if (w.last_doc < L) { w.pos = 0; w.len = 0; }  // refill (with directory skip) next pass
-          else { const uint32_t p = lower_bound128(M.docs + tid * 128, L); if (p > w.pos) w.pos = min(p, w.len); }
-        }
-        __syncthreads();
-        if (dead) continue;
-      }
-    }
-    // (2) the round's bound
-    uint32_t bound = 0xFFFFFFFFu; bool any = false, all = true;
-    for (uint32_t s = 0; s < T; s++) { const TermState& t = M.st[s]; if (!t.done) { bound = min(bound, t.last_doc); any = true; } else all = false; }
-    if (!any || (MODE == 0 && !all)) break;
-    // (3) per-term ranges [pos, hi): docs <= bound
-    if (tid < T) {
-      const TermState& t = M.st[tid];
-      uint32_t hi = t.pos;
-      if (!t.done) { hi = lower_bound128(M.docs + tid * 128, bound + 1u); if (hi > t.len) hi = t.len; if (bound == 0xFFFFFFFFu) hi = t.len; }
-      s_rhi[tid] = hi;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      uint32_t acc = 0;
-      for (uint32_t s = 0; s < T; s++) { s_rstart[s] = acc; if (MODE != 0 || s == 0) acc += s_rhi[s] - M.st[s].pos; }
-      s_rstart[T] = acc;
-    }
-    __syncthreads();
-    const uint32_t R = s_rstart[T];
-    if (*s_count + R > P.cap) {  // make room: keep the best k (TopNComputer::truncate_top_n)
-      sort_keys_desc(M, P.cap);
-      if (tid == 0) {
-        const uint32_t c = min(*s_count, P.k);
-        *s_count = c;
-        if (c == P.k) { *s_flag = 1; *s_thr_hi = M.khi[P.k - 1]; *s_thr_lo = M.klo[P.k - 1]; }
-      }
-      __syncthreads();
-      for (uint32_t i = P.k + tid; i < P.cap; i += NT) { M.khi[i] = 0; M.klo[i] = 0; }
-      __syncthreads();
-    }
-    uint32_t cutoff = 0xFFFFFFFFu;  // path B short circuit: largest doc still inside max_docs
-    bool last_round = false;
-    if (MODE == 2 && P.max_docs) {
-      // count this round's owners; if they overflow max_docs, find the doc cutoff by sorting them
-      uint32_t mine = 0;
-      for (uint32_t e = tid; e < R; e += NT) {
-        uint32_t i = 0; while (e >= s_rstart[i + 1]) i++;
-        const uint32_t d = M.docs[i * 128 + M.st[i].pos + (e - s_rstart[i])];
-        bool owner = true;
-        for (uint32_t x = 0; x < i && owner; x++) if (!M.st[x].done) { const uint32_t j = lower_bound128(M.docs + x * 128, d); if (j < M.st[x].len && M.docs[x * 128 + j] == d) owner = false; }
-        mine += owner;
-      }
-      const uint32_t incl = cta_scan_incl(mine, M.misc);
-      const uint32_t round_owners = __shfl_sync(0xffffffffu, incl, 31);  // lane 31 of the last warp has the total...
-      __syncthreads();
-      if (tid == NT - 1) M.misc[4] = incl;
-      __syncthreads();
-      const uint32_t total_owners = M.misc[4]; (void)round_owners;
-      if (cand_seen + total_owners >= P.max_docs) {
-        last_round = true;
-        const uint32_t remaining = P.max_docs - cand_seen;
-        // owners' docs -> vals/stage scratch is too small for 1024; reuse the (sorted, truncated) tail of the key buffer?  simpler:
-        // select the `remaining`-th smallest owner doc by counting: binary search on the doc value
-        uint32_t lo = 0, hi = bound;
-        while (lo < hi) {
-          const uint32_t mid = lo + ((hi - lo) >> 1);
-          uint32_t c = 0;
-          for (uint32_t e = tid; e < R; e += NT) {
-            uint32_t i = 0; while (e >= s_rstart[i + 1]) i++;
-            const uint32_t d = M.docs[i * 128 + M.st[i].pos + (e - s_rstart[i])];
-            if (d > mid) continue;
-            bool owner = true;
-            for (uint32_t x = 0; x < i && owner; x++) if (!M.st[x].done) { const uint32_t j = lower_bound128(M.docs + x * 128, d); if (j < M.st[x].len && M.docs[x * 128 + j] == d) owner = false; }
-            c += owner;
-          }
-          const uint32_t inc2 = cta_scan_incl(c, M.misc);
-          __syncthreads();
-          if (tid == NT - 1) M.misc[4] = inc2;
-          __syncthreads();
-          if (M.misc[4] >= remaining) hi = mid; else lo = mid + 1;
-          __syncthreads();
-        }
-        cutoff = lo;
-      }
-      cand_seen += total_owners;
-    }
-    // (4) score the round's postings
-    const bool thr_on = *s_flag != 0; const uint64_t thr_hi = *s_thr_hi; const uint32_t thr_lo = *s_thr_lo;
-    for (uint32_t e = tid; e < R; e += NT) {
-      uint32_t i = 0; while (e >= s_rstart[i + 1]) i++;
-      const uint32_t j = M.st[i].pos + (e - s_rstart[i]);
-      const uint32_t d = M.docs[i * 128 + j];
-      if (d > cutoff) continue;
-      uint32_t tf[MAXT];
-      bool ok = true;
-#pragma unroll
-      for (uint32_t x = 0; x < MAXT; x++) {
-        tf[x] = 0;
-        if (x >= T || !ok) continue;
-        if (x == i) { tf[x] = M.tfs[i * 128 + j]; continue; }
-        bool found = false;
-        if (!M.st[x].done) {
-          const uint32_t jj = lower_bound128(M.docs + x * 128, d);
-          if (jj < M.st[x].len && M.docs[x * 128 + jj] == d) { found = true; tf[x] = M.tfs[x * 128 + jj]; }
-        }
-        if (MODE == 0) { if (!found) ok = false; }
-        else if (found && x < i) ok = false;  // a lower slot owns this doc
-      }
-      if (!ok) continue;
-      if (d >= S.max_doc) { bad_doc = 1u; continue; }  // corrupt deltas: never index the doc tables with it
-      my_docs++;
-      const uint32_t fid = S.fieldnorm[d];
-      const float norm = M.cache[fid];
-      uint64_t khi;
-      if (MODE == 2) {
-        float bm = 0.0f;  // MultiBm25Weight::score: f32 sum over the query terms in query order (bm25.rs:97-102)
-#pragma unroll
-        for (uint32_t x = 0; x < MAXT; x++) if (x < T) {
-          float sc = 0.0f;
-          if (tf[x]) { const float t = (float)tf[x]; sc = __fmul_rn(M.st[x].weight, __fdiv_rn(__fmul_rn(t, P.k1p1), __fadd_rn(t, norm))); }
-          bm = __fadd_rn(bm, sc);
-        }
-        double total = __dadd_rn(0.0, __dmul_rn(P.coeff_text, (double)bm));  // initial.rs:80-85: sum of coefficient * score
-        for (uint32_t c = 0; c < P.n_cols; c++) total = __dadd_rn(total, __dmul_rn(P.coeffs[c], P.sig[(size_t)d * P.n_cols + c]));
-        khi = ord_f64(total);
-      } else {
-        float sc[MAXT];
-#pragma unroll
-        for (uint32_t x = 0; x < MAXT; x++) { sc[x] = 0.0f; if (x < T && tf[x]) { const float t = (float)tf[x]; sc[x] = __fmul_rn(M.st[x].weight, __fdiv_rn(t, __fadd_rn(t, norm))); } }
-        float total;
-        if (MODE == 0) {  // Intersection::score = left + right + sum(others) (intersection.rs:153-157)
-          if (T == 1) total = sc[0];
-          else {
-            float others = 0.0f;
-#pragma unroll
-            for (uint32_t x = 2; x < MAXT; x++) if (x < T) others = __fadd_rn(others, sc[x]);
-            total = __fadd_rn(__fadd_rn(sc[0], sc[1]), others);
-          }
-        } else {
-          total = 0.0f;
-#pragma unroll
-          for (uint32_t x = 0; x < MAXT; x++) if (x < T && tf[x]) total = __fadd_rn(total, sc[x]);
-        }
-        khi = (uint64_t)ord_f32(total) << 32;
-      }
-      const uint32_t klo = ~d;
-      if (thr_on && !key_gt(khi, klo, thr_hi, thr_lo)) continue;
-      const uint32_t at = atomicAdd(s_count, 1u);
-      M.khi[at] = khi; M.klo[at] = klo;
-    }
-    __syncthreads();
-    if (tid < T && !M.st[tid].done && (MODE != 0 || true)) M.st[tid].pos = s_rhi[tid];
-    __syncthreads();
-    if (last_round) break;
-  }
-  // final: sort and emit the best k
-  sort_keys_desc(M, P.cap);
-  const uint32_t n = min(*s_count, P.k);
-  for (uint32_t i = tid; i < n; i += NT) {
-    P.o_docs[(size_t)oq * P.k + i] = ~M.klo[i];
-    if (MODE == 2) P.o_totals[(size_t)oq * P.k + i] = unord_f64(M.khi[i]);
-    else P.o_scores[(size_t)oq * P.k + i] = unord_f32((uint32_t)(M.khi[i] >> 32));
-  }
-  if (tid == 0) P.o_n[oq] = n;
-  if (bad_doc) atomicAdd(P.counters + 2, 1ull);  // a decoded doc id outside the segment: reported like a decode failure
-  for (int o = 16; o; o >>= 1) { my_docs += __shfl_down_sync(0xffffffffu, my_docs, o); }
-  if ((tid & 31) == 0 && my_docs) atomicAdd(P.counters + 0, my_docs);
-  if (tid == 0 && my_blocks) atomicAdd(P.counters + 1, my_blocks);
-}
 
 __global__ void k_interleave_signals(const double* const* cols, uint32_t n_cols, uint32_t max_doc, double* rows) {
   const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -621,23 +223,6 @@ __global__ void k_numeric_score(uint32_t kind, uint32_t dtype, const void* __res
     default: break;
   }
   rows[(size_t)d * n_cols + c] = s;
-}
-
-static size_t smem_bytes(uint32_t cap) {
-  return (size_t)cap * 12 + sizeof(TermState) * MAXT + MAXT * 128 * 8 + 344 * 4 + 256 * 4 + 256 * 4 + 40 * 4;
-}
-
-template <int MODE>
-static int launch_topk(const Params& P, uint32_t n_queries, cudaStream_t s) {
-  const size_t sm = smem_bytes(P.cap);
-  static size_t configured[3] = {0, 0, 0};
-  if (sm > 48 * 1024 && configured[MODE] < sm) {
-    SB_CUDA(cudaFuncSetAttribute(k_topk<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    configured[MODE] = sm;
-  }
-  SB_LAUNCH(k_topk<MODE>, n_queries, NT, sm, s, P);
-  SB_CHECK_LAUNCH();
-  return SB200_OK;
 }
 
 template <class T>
@@ -780,7 +365,7 @@ static int run_multi(const sb200_multi_signal_batch* b, uint32_t* docs, double* 
     ns[slot] = c; work_sorted[slot] = work[q];
   }
   ItemPlan pl;
-  plan_items(work_sorted, order, k, g->max_doc, getenv("SB200_BM25_NOSPLIT") == nullptr, pl);
+  plan_items(work_sorted, order, k, g->max_doc, true, pl);
   const uint32_t n_items = (uint32_t)pl.q.size();
   const size_t n_slots_out = (size_t)nq + pl.extra;
   uint32_t cap = 1024; while (cap < k + SM * 128u) cap <<= 1;
@@ -853,23 +438,15 @@ static int run_multi(const sb200_multi_signal_batch* b, uint32_t* docs, double* 
 }
 
 // union modes through k_or3, instantiated for the smallest term-count bound that covers the batch
-template <int MODE, int MINB>
-static int launch_or3_occ(const WParams& P, cudaStream_t s) {
-  const unsigned grid = div_up(P.n_items, WQ);
-  void (*kern)(const WParams) = k_or3<MODE, 8, MINB>;
-  if (P.n_terms_max <= 2) kern = k_or3<MODE, 2, MINB>;
-  else if (P.n_terms_max <= 3) kern = k_or3<MODE, 3, MINB>;
-  else if (P.n_terms_max <= 5) kern = k_or3<MODE, 5, MINB>;
-  SB_LAUNCH(kern, grid, WQ * 32, 0, s, P);
-  SB_CHECK_LAUNCH();
-  return SB200_OK;
-}
 template <int MODE>
 static int launch_or3(const WParams& P, cudaStream_t s) {
-  static const int occ = [] { const char* e = getenv("SB200_OR3_OCC"); return e ? atoi(e) : 6; }();
-  if (occ >= 8) return launch_or3_occ<MODE, 8>(P, s);
-  if (occ >= 6) return launch_or3_occ<MODE, 6>(P, s);
-  return launch_or3_occ<MODE, 5>(P, s);
+  void (*kern)(const WParams) = k_or3<MODE, 8>;
+  if (P.n_terms_max <= 2) kern = k_or3<MODE, 2>;
+  else if (P.n_terms_max <= 3) kern = k_or3<MODE, 3>;
+  else if (P.n_terms_max <= 5) kern = k_or3<MODE, 5>;
+  SB_LAUNCH(kern, div_up(P.n_items, WQ), WQ * 32, 0, s, P);
+  SB_CHECK_LAUNCH();
+  return SB200_OK;
 }
 
 // Result tables to the caller.  An AND batch fills a fraction of its [n_queries][k] table (C4: 72 of 1000 entries per
@@ -943,7 +520,7 @@ static int copy_out_tables(sb200_segment* g, uint32_t nq, uint32_t k, uint32_t* 
 // AND batch through the unit kernel: `terms`/`nterms` are the planned clauses per query slot (sorted by doc_freq),
 // results land in g->o_docs / o_scores / o_n at the caller's query index (order[slot]).  Candidate memory is
 // sum(doc_freq of the rarest clause) x 8 B; slots are processed in groups that keep it under a budget.
-static int run_and3(sb200_segment* g, const Params& P, const std::vector<uint32_t>& terms, const std::vector<uint32_t>& nterms,
+static int run_and3(sb200_segment* g, const SegView& S, const std::vector<uint32_t>& terms, const std::vector<uint32_t>& nterms,
                     uint32_t nq, uint32_t nt, uint32_t k, cudaStream_t s) {
   static_assert(sizeof(AUnit) == sizeof(uint4), "AUnit is stored in a uint4 buffer");
   uint64_t budget = (uint64_t)8 << 30;
@@ -984,19 +561,16 @@ static int run_and3(sb200_segment* g, const Params& P, const std::vector<uint32_
       SB_CUDA(cudaMemcpyAsync(g->a3_units.p, units.data(), (size_t)n_units * sizeof(AUnit), cudaMemcpyHostToDevice, s));
       A3Params A;
       memset(&A, 0, sizeof(A));
-      A.S = P.S; A.a128 = g->a_post.p; A.t_aoff = g->t_aoff.p;
-      A.q_terms = P.q_terms; A.q_nterms = P.q_nterms; A.q_weights = P.q_weights; A.cache = P.cache; A.n_terms_max = nt;
+      A.S = S; A.a128 = g->a_post.p; A.t_aoff = g->t_aoff.p;
+      A.q_terms = g->q_terms.p; A.q_nterms = g->q_nterms.p; A.q_weights = g->q_weights.p; A.cache = g->q_cache.p; A.n_terms_max = nt;
       A.units = (const AUnit*)g->a3_units.p; A.n_units = n_units;
       A.cand_off = g->a3_off.p; A.cand_cnt = g->a3_cnt.p; A.c_key = g->a3_key.p; A.c_doc = g->a3_doc.p;
-      A.counters = P.counters;
-      static const int occ = [] { const char* e = getenv("SB200_AND3_OCC"); return e ? atoi(e) : 8; }();
-      if (occ >= 8) SB_LAUNCH(k_and3<8>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
-      else if (occ >= 6) SB_LAUNCH(k_and3<6>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
-      else SB_LAUNCH(k_and3<5>, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
+      A.counters = g->counters.p;
+      SB_LAUNCH(k_and3, div_up(n_units, A3_WARPS), A3_WARPS * 32, 0, s, A);
       SB_CHECK_LAUNCH();
     }
-    SB_LAUNCH(k_and3_select, g1 - g0, 256, sel_smem, s, g->a3_off.p, g->a3_cnt.p, g->a3_key.p, g->a3_doc.p, P.q_orig, g0, k,
-              P.o_docs, P.o_scores, P.o_n);
+    SB_LAUNCH(k_and3_select, g1 - g0, 256, sel_smem, s, g->a3_off.p, g->a3_cnt.p, g->a3_key.p, g->a3_doc.p, g->q_orig.p, g0, k,
+              g->o_docs.p, g->o_scores.p, g->o_n.p);
     SB_CHECK_LAUNCH();
     if (g1 < nq) SB_CUDA(cudaStreamSynchronize(s));  // `units` / `off` are reused by the next group's async copies
     g0 = g1;
@@ -1020,6 +594,7 @@ static int run_batch(sb200_segment* g, const sb200_bm25_batch* b, int mode, cons
   // longest-processing-time-first: one warp walks a whole query, so the batch finishes when its largest query
   // does; slots are ordered by decreasing posting count and results go back to the caller's index (q_orig)
   std::vector<uint32_t> order(nq);
+  std::vector<uint64_t> slot_work(nq, 0);   // postings per query slot
   {
     std::vector<uint64_t> work(nq, 0);
     for (uint32_t q = 0; q < nq; q++) {
@@ -1041,80 +616,43 @@ static int run_batch(sb200_segment* g, const sb200_bm25_batch* b, int mode, cons
     for (uint32_t i = 0; i < c; i++) {
       terms[(size_t)slot * nt + i] = b->term_ords[(size_t)q * nt + idx[i]];
       weights[(size_t)slot * nt + i] = b->weights[(size_t)q * nt + idx[i]];
-      postings += g->h_df[terms[(size_t)slot * nt + i]];
+      slot_work[slot] += g->h_df[terms[(size_t)slot * nt + i]];
     }
+    postings += slot_work[slot];
     nterms[slot] = c;
   }
-  // work items: queries much larger than the average are cut into doc ranges (<= 16, W*k <= 16384 for the merge)
-  std::vector<uint32_t> it_q, it_lo, it_hi, it_out;
-  std::vector<MergeJob> jobs;
-  uint32_t extra = 0, capm = 0;
-  {
-    const bool can_split = !(sb && sb->max_docs) && !(!sb && mode == SB200_MODE_OR_WAND) && getenv("SB200_BM25_CTA") == nullptr &&
-                           getenv("SB200_BM25_NOSPLIT") == nullptr;   // a replayed history cannot be cut into doc ranges
-    const uint64_t target = std::max<uint64_t>(32768, postings / std::max<uint32_t>(nq, 1));
-    const uint32_t wmax = std::max<uint32_t>(1, std::min<uint32_t>(16, 16384 / k));
-    it_q.reserve(nq + 64); it_lo.reserve(nq + 64); it_hi.reserve(nq + 64); it_out.reserve(nq + 64);
-    for (uint32_t slot = 0; slot < nq; slot++) {
-      uint64_t work = 0;
-      for (uint32_t i = 0; i < nterms[slot]; i++) work += g->h_df[terms[(size_t)slot * nt + i]];
-      uint32_t W = can_split ? (uint32_t)std::min<uint64_t>(wmax, (work + target - 1) / target) : 1;
-      if (W < 1) W = 1;
-      if (W == 1) { it_q.push_back(slot); it_lo.push_back(0); it_hi.push_back(0xFFFFFFFFu); it_out.push_back(order[slot]); continue; }
-      MergeJob j; j.first_slot = nq + extra; j.n_slots = W; j.out_slot = order[slot]; j._pad = 0;
-      jobs.push_back(j);
-      for (uint32_t c = 0; c < W; c++) {
-        it_q.push_back(slot);
-        it_lo.push_back((uint32_t)((uint64_t)g->max_doc * c / W));
-        it_hi.push_back(c + 1 == W ? 0xFFFFFFFFu : (uint32_t)((uint64_t)g->max_doc * (c + 1) / W));
-        it_out.push_back(nq + extra + c);
-      }
-      extra += W;
-    }
-    if (!jobs.empty()) { capm = 1024; while (capm < wmax * k) capm <<= 1; }
-  }
-  const uint32_t n_items = (uint32_t)it_q.size();
-  const size_t n_slots_out = (size_t)nq + extra;
+  ItemPlan pl;   // a replayed history (Block-WAND) and the max_docs short circuit cannot be cut into doc ranges
+  plan_items(slot_work, order, k, g->max_doc, !(sb && sb->max_docs) && !(!sb && mode == SB200_MODE_OR_WAND), pl);
+  const uint32_t n_items = (uint32_t)pl.q.size();
+  const size_t n_slots_out = (size_t)nq + pl.extra;
   SB_TRY(ensure(g->q_terms, (size_t)nq * nt)); SB_TRY(ensure(g->q_weights, (size_t)nq * nt)); SB_TRY(ensure(g->q_nterms, nq));
   SB_TRY(ensure(g->q_cache, 256)); SB_TRY(ensure(g->o_docs, n_slots_out * k)); SB_TRY(ensure(g->o_n, n_slots_out));
   if (totals) SB_TRY(ensure(g->o_totals, n_slots_out * k)); else SB_TRY(ensure(g->o_scores, n_slots_out * k));
   SB_TRY(ensure(g->counters, 4)); SB_TRY(ensure(g->q_orig, nq));
-  SB_TRY(ensure(g->q_items, (size_t)4 * n_items)); SB_TRY(ensure(g->q_jobs, jobs.size() + 1));
+  SB_TRY(ensure(g->q_items, (size_t)4 * n_items)); SB_TRY(ensure(g->q_jobs, pl.jobs.size() + 1));
   SB_CUDA(cudaEventRecord(g->ev0, s));
   SB_CUDA(cudaMemcpyAsync(g->q_orig.p, order.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
-  SB_CUDA(cudaMemcpyAsync(g->q_items.p, it_q.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
-  SB_CUDA(cudaMemcpyAsync(g->q_items.p + n_items, it_lo.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
-  SB_CUDA(cudaMemcpyAsync(g->q_items.p + 2 * (size_t)n_items, it_hi.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
-  SB_CUDA(cudaMemcpyAsync(g->q_items.p + 3 * (size_t)n_items, it_out.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
-  if (!jobs.empty()) SB_CUDA(cudaMemcpyAsync(g->q_jobs.p, jobs.data(), jobs.size() * sizeof(MergeJob), cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_items.p, pl.q.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_items.p + n_items, pl.lo.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_items.p + 2 * (size_t)n_items, pl.hi.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemcpyAsync(g->q_items.p + 3 * (size_t)n_items, pl.out.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice, s));
+  if (!pl.jobs.empty()) SB_CUDA(cudaMemcpyAsync(g->q_jobs.p, pl.jobs.data(), pl.jobs.size() * sizeof(MergeJob), cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->q_terms.p, terms.data(), terms.size() * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->q_weights.p, weights.data(), weights.size() * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, nterms.data(), nterms.size() * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->q_cache.p, b->tf_cache256, 256 * 4, cudaMemcpyDefault, s));
   SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 4 * sizeof(unsigned long long), s));
-  Params P;
-  memset(&P, 0, sizeof(P));
-  P.S.p32 = (const uint32_t*)g->postings.p; P.S.postings_len = g->postings_len; P.S.fieldnorm = g->fieldnorm.p; P.S.max_doc = g->max_doc;
-  P.S.t_data_off = g->t_data_off.p; P.S.t_end_off = g->t_end_off.p; P.S.t_df = g->t_df.p; P.S.t_first = g->t_first.p;
-  P.S.b_last = g->b_last.p; P.S.b_off = g->b_off.p; P.S.b_bits = g->b_bits.p; P.S.record = g->record;
-  P.q_terms = g->q_terms.p; P.q_nterms = g->q_nterms.p; P.q_weights = g->q_weights.p; P.cache = g->q_cache.p; P.q_orig = g->q_orig.p;
-  P.n_terms_max = nt; P.k = k;
-  uint32_t cap = 1024; while (cap < k + nt * 128u) cap <<= 1;
-  P.cap = cap;
-  P.o_docs = g->o_docs.p; P.o_scores = g->o_scores.p; P.o_totals = g->o_totals.p; P.o_n = g->o_n.p; P.counters = g->counters.p;
+  SegView S;
+  seg_view(g, S);
   SB_CUDA(cudaEventRecord(g->evk0, s));
-  if (sb) {
-    P.k1p1 = sb->k1 + 1.0f;  // constants.k1 + 1.0 in f32 (core/src/ranking/bm25.rs:149)
-    P.coeff_text = sb->coeff_text; P.max_docs = sb->max_docs;
-    if (sb->signals && sb->signals->n_cols) {
-      if (sb->signals->max_doc < g->max_doc) SB_FAIL(SB200_EINVAL, "signal table covers %u docs, segment has %u", sb->signals->max_doc, g->max_doc);
-      if (!sb->coeffs) SB_FAIL(SB200_EINVAL, "coeffs is NULL");
-      SB_TRY(ensure(g->q_coeffs, sb->signals->n_cols));
-      SB_CUDA(cudaMemcpyAsync(g->q_coeffs.p, sb->coeffs, sb->signals->n_cols * 8, cudaMemcpyDefault, s));
-      P.sig = sb->signals->rows.p; P.n_cols = sb->signals->n_cols; P.coeffs = g->q_coeffs.p;
-    }
-  }
   if (!sb && mode != SB200_MODE_AND && mode != SB200_MODE_OR && mode != SB200_MODE_OR_WAND) SB_FAIL(SB200_EINVAL, "mode %d", mode);
+  // a single-clause "intersection" makes every posting a hit: its candidate list in k_and3 would be the whole posting list
+  // and the select pass would crawl through it chunk by chunk; the threshold-pruning k_topk_warp<AND> handles those batches
+  const bool and_long_single = !sb && mode == SB200_MODE_AND && [&] {
+    for (uint32_t slot = 0; slot < nq; slot++)
+      if (nterms[slot] == 1 && g->h_df[terms[(size_t)slot * nt]] > 65536u) return true;
+    return false;
+  }();
   if (!sb && mode == SB200_MODE_OR_WAND) {
     // block_wand replayed (bm25_wand.cuh): one warp per query slot, the reference's own pruning and summation order
     if (g->record < 1) SB_FAIL(SB200_EINVAL, "Block-WAND needs term frequencies (record option WithFreqs or above)");
@@ -1122,54 +660,50 @@ static int run_batch(sb200_segment* g, const sb200_bm25_batch* b, int mode, cons
     SB_TRY(ensure(g->g_khi, (size_t)nq * wcap)); SB_TRY(ensure(g->g_klo, (size_t)nq * wcap));
     WandParams W;
     memset(&W, 0, sizeof(W));
-    W.S = P.S; W.b_bw = g->b_bw.p; W.a128 = g->a_post.p; W.t_aoff = g->t_aoff.p;
-    W.q_terms = P.q_terms; W.q_nterms = P.q_nterms; W.q_weights = P.q_weights; W.cache = P.cache; W.q_orig = P.q_orig;
+    W.S = S; W.b_bw = g->b_bw.p; W.a128 = g->a_post.p; W.t_aoff = g->t_aoff.p;
+    W.q_terms = g->q_terms.p; W.q_nterms = g->q_nterms.p; W.q_weights = g->q_weights.p; W.cache = g->q_cache.p; W.q_orig = g->q_orig.p;
     W.n_queries = nq; W.n_terms_max = nt; W.k = k; W.cap = wcap;
-    W.g_khi = g->g_khi.p; W.g_klo = g->g_klo.p; W.o_docs = P.o_docs; W.o_scores = P.o_scores; W.o_n = P.o_n; W.counters = P.counters;
+    W.g_khi = g->g_khi.p; W.g_klo = g->g_klo.p; W.o_docs = g->o_docs.p; W.o_scores = g->o_scores.p; W.o_n = g->o_n.p; W.counters = g->counters.p;
     SB_LAUNCH(k_wand, div_up(nq, WD_WARPS), WD_WARPS * 32, 0, s, W);
     SB_CHECK_LAUNCH();
+  } else if (!sb && mode == SB200_MODE_AND && !and_long_single) {
+    SB_TRY(run_and3(g, S, terms, nterms, nq, nt, k, s));
   } else {
-  const int kmode = sb ? 2 : mode;
-  static const bool use_cta_kernel = getenv("SB200_BM25_CTA") != nullptr;  // the first-generation CTA-per-query kernel
-  if (use_cta_kernel) {
-    if (kmode == 2) SB_TRY(launch_topk<2>(P, nq, s));
-    else if (kmode == 0) SB_TRY(launch_topk<0>(P, nq, s));
-    else SB_TRY(launch_topk<1>(P, nq, s));
-  } else if (kmode == 0 && env_flag("SB200_BM25_AND3", true) && [&] {
-               // a single-clause "intersection" makes every posting a hit: its candidate list is the whole posting list and
-               // the select pass would crawl through it chunk by chunk; the threshold-pruning kernel handles those batches
-               for (uint32_t slot = 0; slot < nq; slot++)
-                 if (nterms[slot] == 1 && g->h_df[terms[(size_t)slot * nt]] > 65536u) return false;
-               return true;
-             }()) {
-    SB_TRY(run_and3(g, P, terms, nterms, nq, nt, k, s));  // unit-based intersection (bm25_and3.cuh); SB200_BM25_AND3=0: k_topk_warp<AND>
-  } else {
+    // the walk kernels: k_or3 for OR and the signal combine, k_topk_warp for the batches it does not cover
+    uint32_t cap = 1024; while (cap < k + nt * 128u) cap <<= 1;
     SB_TRY(ensure(g->g_khi, (size_t)n_items * cap)); SB_TRY(ensure(g->g_klo, (size_t)n_items * cap));
     WParams W;
     memset(&W, 0, sizeof(W));
-    W.S = P.S; W.a128 = g->a_post.p; W.t_aoff = g->t_aoff.p;
-    W.q_terms = P.q_terms; W.q_nterms = P.q_nterms; W.q_weights = P.q_weights; W.cache = P.cache; W.q_orig = P.q_orig;
+    W.S = S; W.a128 = g->a_post.p; W.t_aoff = g->t_aoff.p;
+    W.q_terms = g->q_terms.p; W.q_nterms = g->q_nterms.p; W.q_weights = g->q_weights.p; W.cache = g->q_cache.p; W.q_orig = g->q_orig.p;
     W.n_queries = nq; W.n_terms_max = nt; W.k = k; W.cap = cap;
     W.n_items = n_items; W.item_q = g->q_items.p; W.item_lo = g->q_items.p + n_items; W.item_hi = g->q_items.p + 2 * (size_t)n_items; W.item_out = g->q_items.p + 3 * (size_t)n_items;
-    W.k1p1 = P.k1p1; W.coeff_text = P.coeff_text; W.sig = P.sig; W.n_cols = P.n_cols; W.coeffs = P.coeffs; W.max_docs = P.max_docs;
     W.g_khi = g->g_khi.p; W.g_klo = g->g_klo.p;
-    W.o_docs = P.o_docs; W.o_scores = P.o_scores; W.o_totals = P.o_totals; W.o_n = P.o_n; W.counters = P.counters;
-    W.use_tma = env_flag("SB200_BM25_TMA", true) ? 1u : 0u;
-    const bool use_or3 = kmode != 0 && W.max_docs == 0 && env_flag("SB200_BM25_OR3", true);  // bm25_or3.cuh; SB200_BM25_OR3=0: k_topk_warp
-    if (use_or3) { if (kmode == 2) SB_TRY(launch_or3<2>(W, s)); else SB_TRY(launch_or3<1>(W, s)); }
-    else if (kmode == 2) SB_TRY(launch_topk_warp<2>(W, s));
-    else if (kmode == 0) SB_TRY(launch_topk_warp<0>(W, s));
-    else SB_TRY(launch_topk_warp<1>(W, s));
-    if (!jobs.empty()) {
-      const size_t msm = (size_t)capm * 12;
+    W.o_docs = g->o_docs.p; W.o_scores = g->o_scores.p; W.o_totals = g->o_totals.p; W.o_n = g->o_n.p; W.counters = g->counters.p;
+    if (sb) {
+      W.k1p1 = sb->k1 + 1.0f;  // constants.k1 + 1.0 in f32 (core/src/ranking/bm25.rs:149)
+      W.coeff_text = sb->coeff_text; W.max_docs = sb->max_docs;
+      if (sb->signals && sb->signals->n_cols) {
+        if (sb->signals->max_doc < g->max_doc) SB_FAIL(SB200_EINVAL, "signal table covers %u docs, segment has %u", sb->signals->max_doc, g->max_doc);
+        if (!sb->coeffs) SB_FAIL(SB200_EINVAL, "coeffs is NULL");
+        SB_TRY(ensure(g->q_coeffs, sb->signals->n_cols));
+        SB_CUDA(cudaMemcpyAsync(g->q_coeffs.p, sb->coeffs, sb->signals->n_cols * 8, cudaMemcpyDefault, s));
+        W.sig = sb->signals->rows.p; W.n_cols = sb->signals->n_cols; W.coeffs = g->q_coeffs.p;
+      }
+    }
+    if (!sb && mode == SB200_MODE_AND) SB_TRY(launch_topk_warp<0>(W, s));
+    else if (sb && sb->max_docs) SB_TRY(launch_topk_warp<2>(W, s));   // k_or3 has no max_docs short circuit
+    else if (sb) SB_TRY(launch_or3<2>(W, s));
+    else SB_TRY(launch_or3<1>(W, s));
+    if (!pl.jobs.empty()) {
+      const size_t msm = (size_t)pl.capm * 12;
       static size_t mconf[3] = {0, 0, 0};
-      if (kmode == 2) { if (msm > 48 * 1024 && mconf[2] < msm) { SB_CUDA(cudaFuncSetAttribute(k_merge_topk<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); mconf[2] = msm; }
-                        SB_LAUNCH(k_merge_topk<2>, (unsigned)jobs.size(), 256, msm, s, g->q_jobs.p, k, capm, P.o_docs, P.o_scores, P.o_totals, P.o_n); }
+      if (sb) { if (msm > 48 * 1024 && mconf[2] < msm) { SB_CUDA(cudaFuncSetAttribute(k_merge_topk<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); mconf[2] = msm; }
+                SB_LAUNCH(k_merge_topk<2>, (unsigned)pl.jobs.size(), 256, msm, s, g->q_jobs.p, k, pl.capm, W.o_docs, W.o_scores, W.o_totals, W.o_n); }
       else { if (msm > 48 * 1024 && mconf[0] < msm) { SB_CUDA(cudaFuncSetAttribute(k_merge_topk<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); mconf[0] = msm; }
-             SB_LAUNCH(k_merge_topk<0>, (unsigned)jobs.size(), 256, msm, s, g->q_jobs.p, k, capm, P.o_docs, P.o_scores, P.o_totals, P.o_n); }
+             SB_LAUNCH(k_merge_topk<0>, (unsigned)pl.jobs.size(), 256, msm, s, g->q_jobs.p, k, pl.capm, W.o_docs, W.o_scores, W.o_totals, W.o_n); }
       SB_CHECK_LAUNCH();
     }
-  }
   }
   SB_CUDA(cudaEventRecord(g->evk1, s));
   SB_TRY(copy_out_tables(g, nq, k, docs, scores, totals, n_out));

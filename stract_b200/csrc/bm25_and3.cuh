@@ -1,5 +1,5 @@
-// bm25_and3.cuh -- AND queries, third generation (the default AND kernel: bit-identical to k_topk_warp<AND>;
-// SB200_BM25_AND3=0 switches back).
+// bm25_and3.cuh -- AND queries, third generation (bit-identical to k_topk_warp<AND>, which keeps only the batches
+// with a single-clause query above 65 536 postings).
 //
 // Why: a CPU emulation of k_topk_warp<AND> on the C4 batch (10k 2-term queries) counts 4.1 M rounds of ~250 per
 // work item, evenly spread -- no tail -- and a round there is ~1500
@@ -161,10 +161,9 @@ __device__ __forceinline__ float a3_term_score(float weight, uint32_t tf, float 
   return __fmul_rn(weight, __fdiv_rn(t, __fadd_rn(t, norm)));   // Bm25Weight::score, bm25.rs:182-196
 }
 
-// MINB = resident CTAs per SM the register allocation aims for (5: 96 registers, no spill; 6: 80; 8: 64 with a small spill).
-// The kernel lives on latency hiding, so 8 is the default (SB200_AND3_OCC selects).
-template <int MINB>
-__global__ void __launch_bounds__(A3_WARPS * 32, MINB) k_and3(const A3Params P) {
+// At least 8 resident CTAs per SM caps the registers at 64, with a small spill (5 CTAs would allow 96 and no spill,
+// 6 would allow 80).  The kernel lives on latency hiding, so occupancy wins.
+__global__ void __launch_bounds__(A3_WARPS * 32, 8) k_and3(const A3Params P) {
   __shared__ float cache[256];
   __shared__ __align__(16) uint32_t s_docs[A3_WARPS][128];
   __shared__ __align__(16) uint32_t s_tfs[A3_WARPS][128];

@@ -1,5 +1,5 @@
-// bm25_or3.cuh -- OR / signal-combine queries, third generation (the default union kernel since round 2: bit-identical
-// to k_topk_warp<OR|SIGNAL> on hardware, 1.2-1.4x faster; SB200_BM25_OR3=0 switches back).
+// bm25_or3.cuh -- OR / signal-combine queries, third generation (the union kernel since round 2: bit-identical
+// to k_topk_warp<OR|SIGNAL> on hardware, 1.2-1.4x faster).
 //
 // Same algorithm, work items, candidate buffers, merge pass and bit-exact scoring as k_topk_warp (block-synchronous
 // union: bound = smallest last-doc of the current blocks, lowest slot owns a doc, TopNComputer-style threshold),
@@ -129,10 +129,10 @@ __device__ uint32_t o3_decode(const SegView& S, const uint4* __restrict__ a128, 
 }
 
 // MODE 1: OR (tantivy weights, query-order f32 sum), MODE 2: Stract BM25 + f64 linear signal combine
-// MINB: resident CTAs per SM the register allocation aims for (5 => 96 registers, 6 => 80, 8 => 64 with a small spill);
-// the kernel is latency-bound, so occupancy is what the choice trades against spills
-template <int MODE, int TMAX, int MINB>
-__global__ void __launch_bounds__(WQ * 32, MINB) k_or3(const WParams P) {
+// At least 6 resident CTAs per SM caps the registers at 80 (5 would allow 96; 8 would cap them at 64 and spill); the
+// kernel is latency-bound, so occupancy is what the choice trades against spills
+template <int MODE, int TMAX>
+__global__ void __launch_bounds__(WQ * 32, 6) k_or3(const WParams P) {
   static_assert(MODE == 1 || MODE == 2, "k_or3 covers the union modes");
   __shared__ float cache[256];
   __shared__ __align__(16) uint32_t s_docs[WQ][TMAX * 128];
@@ -168,13 +168,10 @@ __global__ void __launch_bounds__(WQ * 32, MINB) k_or3(const WParams P) {
   uint32_t my_pos = 0, my_len = 0, my_last = 0, my_cur = 0, my_prev = 0;
   bool my_done = true, my_tail_done = false;
   uint32_t my_pf = O3_NONE, my_phase = 0;   // block whose bytes are (being) staged for this lane's term; parity to wait for
-  const bool use_tma = P.use_tma != 0;
   uint64_t* bar = s_bar[warp];
-  if (use_tma) {
-    if (lane < TMAX) mbar_init(bar + lane, 1);
-    mbar_fence_init();
-    __syncwarp();
-  }
+  if (lane < TMAX) mbar_init(bar + lane, 1);
+  mbar_fence_init();
+  __syncwarp();
   unsigned long long budget = 64;
   if (lane < T) {
     OTerm c;
@@ -225,17 +222,15 @@ __global__ void __launch_bounds__(WQ * 32, MINB) k_or3(const WParams P) {
         }
         uint32_t last;
         const uint4* staged = nullptr;
-        if (use_tma) {
-          const uint32_t pf = __shfl_sync(0xffffffffu, my_pf, s), ph = __shfl_sync(0xffffffffu, my_phase, s);
-          if (pf != O3_NONE) {               // an outstanding copy is always waited for before its buffer / barrier is reused
-            mbar_wait(bar + s, ph);
-            if (pf == cur) staged = (const uint4*)s_stage[warp][s];
-            if (lane == (uint32_t)s) { my_pf = O3_NONE; my_phase ^= 1u; }
-          }
+        const uint32_t pf = __shfl_sync(0xffffffffu, my_pf, s), ph = __shfl_sync(0xffffffffu, my_phase, s);
+        if (pf != O3_NONE) {               // an outstanding copy is always waited for before its buffer / barrier is reused
+          mbar_wait(bar + s, ph);
+          if (pf == cur) staged = (const uint4*)s_stage[warp][s];
+          if (lane == (uint32_t)s) { my_pf = O3_NONE; my_phase ^= 1u; }
         }
         const uint32_t n = o3_decode(S, P.a128, c, cur, prev, docs + s * 128, tfs + s * 128, bloom + s * 16, lane, last, staged);
         my_blocks++;
-        if (use_tma && cur + 1 < c.nfull) {  // o3_decode ended with a warp barrier: every lane is done with the staging buffer
+        if (cur + 1 < c.nfull) {  // o3_decode ended with a warp barrier: every lane is done with the staging buffer
           uint32_t issued = 0;
           if (lane == 0) {
             const uint32_t idx = c.first + cur + 1, bits = S.b_bits[idx];
@@ -369,7 +364,7 @@ __global__ void __launch_bounds__(WQ * 32, MINB) k_or3(const WParams P) {
     }
     __syncwarp();
   }
-  if (use_tma && my_pf != O3_NONE) mbar_wait(bar + lane, my_phase);   // no copy may still be in flight when the warp leaves
+  if (my_pf != O3_NONE) mbar_wait(bar + lane, my_phase);   // no copy may still be in flight when the warp leaves
   __threadfence_block();
   __syncwarp();
   w_sort_prefix_desc(khi, klo, *s_count, P.cap, lane);

@@ -1,16 +1,17 @@
 // bm25_warp.cuh -- k_topk_warp<MODE>: one WARP per query (4 queries per 128-thread CTA), no block barriers.
 //
-// Same algorithm and bit-exact scoring as k_topk (bm25.cu) -- block-synchronous walk of the query terms'
-// posting lists, `bound` = smallest last-doc of the current blocks, membership by 7-step search in the other
-// terms' decoded blocks, lowest slot owns a doc, exact top-k with a TopNComputer-style threshold -- but laid
-// out for throughput on a 10k-query batch:
+// Serves the batches k_and3 and k_or3 do not (see the header of bm25.cu): AND with a single-clause query above 65 536
+// postings, and the signal combine with max_docs.  Block-synchronous walk of the query terms' posting lists: every
+// round takes `bound` = smallest last-doc of the current blocks (every posting <= bound is final), membership is a
+// 7-step search in the other terms' decoded blocks, the lowest slot containing a doc owns it, and the exact top-k
+// uses a TopNComputer-style threshold (top_score_collector.rs:501-554).  Laid out for throughput on a 10k-query batch:
 //   * a warp decodes a 128-doc BitPacker4x block by itself: lane s owns slot s of the four interleaved lane
 //     streams, i.e. docs 4s..4s+3; the block bytes are read as 16-byte vectors from a 16-byte aligned copy of the
 //     block regions made at segment open (every block is a multiple of 16 bytes), so one LDG.128 returns word w
 //     of all four streams; the strict-delta prefix sum is 3 adds + a 5-step warp scan;
 //   * per-term state and the decoded blocks live in per-warp shared memory (1 KB per term), so ~32 warps =
-//     32 independent queries are resident per SM and hide each other's gather latency -- the CTA-per-query
-//     kernel was bound by barrier and dependent-load latency with only 6 queries per SM;
+//     32 independent queries are resident per SM and hide each other's gather latency -- one CTA per query was
+//     bound by barrier and dependent-load latency with only 6 queries per SM;
 //   * the 2k-entry candidate buffer lives in global memory (L2): pushes are rare once the threshold is up
 //     (~k ln(n/k) per query) and the warp-level bitonic truncation runs a handful of times per query.
 #pragma once
@@ -41,7 +42,6 @@ struct WParams {
   float k1p1; double coeff_text; const double* sig; uint32_t n_cols; const double* coeffs; uint32_t max_docs;
   uint64_t* g_khi; uint32_t* g_klo;   // [n_queries][cap] candidate buffers
   uint32_t* o_docs; float* o_scores; double* o_totals; uint32_t* o_n; unsigned long long* counters;
-  uint32_t use_tma;   // k_or3: stage the next posting block of every term with cp.async.bulk (SB200_BM25_TMA=0 turns it off)
 };
 
 __device__ __forceinline__ uint32_t warp_scan_incl(uint32_t x, uint32_t lane) {
@@ -172,6 +172,7 @@ __device__ __forceinline__ void w_sort_prefix_desc(uint64_t* khi, uint32_t* klo,
 
 template <int MODE>
 __global__ void __launch_bounds__(WQ * 32) k_topk_warp(const WParams P) {
+  static_assert(MODE == 0 || MODE == 2, "k_topk_warp serves AND and the signal combine; OR goes to k_or3");
   SB_DYN_SMEM(smem_raw);
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t TM = P.n_terms_max;

@@ -6,8 +6,8 @@ fill-level race in k_topk_warp was found).  The parity functions are the ones of
 the oracle exactly as on the GPU; this file only swaps the library underneath them.
 
 What this is NOT: a performance statement, a memory-model checker, or part of the product -- stract_b200 never loads
-the emulator; only this test does.  It lets the opt-in kernels (bm25_and3.cuh, bm25_or3.cuh), which were written
-without a GPU at hand, be checked bit-exactly before the first GPU trip."""
+the emulator; only this test does.  It lets kernels written without a GPU at hand, as bm25_and3.cuh and bm25_or3.cuh
+were, be checked bit-exactly before their first GPU run."""
 import ctypes as C
 import os
 import subprocess
@@ -32,8 +32,6 @@ def emulated():
         yield T
     finally:
         _lib._LIB = saved
-        for k in ("SB200_BM25_AND3", "SB200_BM25_OR3", "SB200_AND3_BUDGET_MB"):
-            os.environ.pop(k, None)
 
 
 def test_default_kernels_against_oracle(emulated):
@@ -55,49 +53,14 @@ def test_default_kernels_against_oracle(emulated):
 
 
 def test_unit_based_and_kernel_against_oracle(emulated, monkeypatch):
-    emulated.test_and3_unit_kernel_bit_exact(monkeypatch)   # the skipif mark only gates collection on a GPU box
+    emulated.test_and3_unit_kernel_bit_exact(monkeypatch)
 
 
-def test_union_kernel_matches_default_kernel(emulated, monkeypatch):
-    """A reduced form of test_or3_union_kernel_matches_default_kernel (the full one takes ~10 min emulated): OR with
-    1..8 clauses, absent clauses, doc-range items + merge, signal combine with 4 / 2 / 0 columns."""
-    T = emulated
-    from stract_b200.bm25 import MODE_OR, NO_TERM, SignalComputer, SignalTable, TopDocs
-    dfs = [1, 5, 127, 128, 129, 300, 1000, 1280, 5000, 12000, 20000]
-    (oseg, seg), rng = T.random_index(33, 60_000, dfs)
-    nt = len(dfs)
-
-    def both(fn):
-        monkeypatch.delenv("SB200_BM25_OR3", raising=False)
-        a = fn()
-        monkeypatch.setenv("SB200_BM25_OR3", "1")
-        b = fn()
-        monkeypatch.delenv("SB200_BM25_OR3", raising=False)
-        return a, b
-
-    for width in (1, 2, 3, 5, 8):
-        nq = 24
-        terms = np.stack([rng.choice(nt, width, replace=False) for _ in range(nq)]).astype(np.uint32)
-        if width >= 3:
-            terms[::5, 1] = NO_TERM
-        for k in (1, 100):
-            (ad, as_, an), (bd, bs, bn) = both(lambda: TopDocs.with_limit(k).search_batch(seg, terms, MODE_OR))
-            assert np.array_equal(an, bn), (width, k)
-            for q in range(nq):
-                assert np.array_equal(ad[q, :an[q]], bd[q, :bn[q]]) and np.array_equal(as_[q, :an[q]], bs[q, :bn[q]]), (width, k, q)
-    for ncols in (4, 2, 0):
-        cols = [rng.random(60_000) for _ in range(ncols)]
-        comp = SignalComputer(seg, SignalTable(cols) if ncols else None, [2.0, 0.02, 2.0, 0.001][:ncols], coeff_text=0.005)
-        terms = np.stack([rng.choice(nt, 5, replace=False) for _ in range(16)]).astype(np.uint32)
-        (ad, at, an), (bd, bt, bn) = both(lambda: comp.top_docs_batch(terms, 200))
-        assert np.array_equal(an, bn)
-        for q in range(16):
-            assert np.array_equal(ad[q, :an[q]], bd[q, :bn[q]]) and np.array_equal(at[q, :an[q]], bt[q, :bn[q]]), (ncols, q)
-    # and the union kernel against the oracle directly (not only against the other kernel)
-    monkeypatch.setenv("SB200_BM25_OR3", "1")
-    T.test_or_queries_bit_exact_up_to_two_terms()
-    T.test_or_three_plus_terms_canonical_order()
-    T.test_signal_combine_bit_exact()
+def test_union_kernel_against_oracle(emulated):
+    """A reduced form of test_or3_union_kernel_bit_exact (the full one takes ~10 min emulated): OR with 1..8 clauses,
+    absent clauses, doc-range items + merge, signal combine with 4 / 2 / 0 columns."""
+    emulated.union_kernel_against_oracle(33, 60_000, [1, 5, 127, 128, 129, 300, 1000, 1280, 5000, 12000, 20000],
+                                         nq=24, ks=(1, 100), pad_every=5, sig_nq=16, sig_k=200)
 
 
 def test_multi_field_signals_against_oracle(emulated):

@@ -1,7 +1,5 @@
 """Parity of the CUDA BM25 top-k path (through the C ABI) against the CPU oracle.  Needs a GPU.
 Bar: doc ids, order and f32 scores / f64 totals bit-exact."""
-import os
-
 import numpy as np
 import pytest
 
@@ -86,6 +84,18 @@ def test_and_queries_bit_exact():
     # the two most frequent terms: thousands of matches -> exercises the buffer truncation
     check_query(oseg, seg, [nt - 1, nt - 2], MODE_AND, 100)
     check_query(oseg, seg, [nt - 1, nt - 2, nt - 3], MODE_AND, 1000)
+    # a single clause above 65 536 postings sends its whole batch to k_topk_warp<AND>, the two-clause queries in it too
+    (oseg, seg), _ = random_index(17, 100_000, [70_000, 500])
+    for q in ([0], [0, 1]):
+        for k in (10, 1000):
+            check_query(oseg, seg, q, MODE_AND, k)
+    terms = np.array([[0, NO_TERM], [0, 1], [1, 0]], np.uint32)
+    gd, gs, gn = TopDocs.with_limit(1000).search_batch(seg, terms, MODE_AND)
+    for q in range(len(terms)):
+        qq = np.array([x for x in terms[q] if x != NO_TERM], np.uint32)
+        od, os_, _ = oseg.topk(qq, *weights_for(seg, qq), MODE_AND, 1000)
+        assert gn[q] == len(od), q
+        assert np.array_equal(gd[q, :gn[q]], od) and np.array_equal(gs[q, :gn[q]], os_), q
 
 
 def test_or_queries_bit_exact_up_to_two_terms():
@@ -194,12 +204,10 @@ def test_malformed_postings_rejected():
         SegmentReader(data[:100], (off, ln, df), oseg.fieldnorm_ids)  # term range outside the file
 
 
-@pytest.mark.skipif(not os.environ.get("SB200_TEST_AND3"), reason="unit-based AND kernel (bm25_and3.cuh) is opt-in until it has been run once on a GPU: SB200_TEST_AND3=1")
 def test_and3_unit_kernel_bit_exact(monkeypatch):
-    """The opt-in unit-based intersection must give exactly what the default kernel and the oracle give:
-    ragged clause sizes (tail-only terms, exact multiples of 128), 1..4 clauses, k below/above the hit count,
-    and a budget small enough to force several candidate groups."""
-    monkeypatch.setenv("SB200_BM25_AND3", "1")
+    """The unit-based intersection (bm25_and3.cuh) against the oracle: ragged clause sizes (tail-only terms, exact
+    multiples of 128), 1..4 clauses, k below/above the hit count, and a budget small enough to force several
+    candidate groups."""
     dfs = [1, 5, 127, 128, 129, 255, 256, 300, 1000, 1280, 5000, 20000, 40000]
     (oseg, seg), rng = random_index(21, 80_000, dfs)
     nt = len(dfs)
@@ -229,41 +237,43 @@ def test_and3_unit_kernel_bit_exact(monkeypatch):
     assert st["docs_scored"] == int(on.sum()) or st["docs_scored"] >= int(on.sum())
 
 
-@pytest.mark.skipif(not os.environ.get("SB200_TEST_OR3"), reason="union kernel k_or3 (bm25_or3.cuh) is opt-in until it has been run once on a GPU: SB200_TEST_OR3=1")
-def test_or3_union_kernel_matches_default_kernel(monkeypatch):
-    """Differential test: the opt-in union kernel must return exactly what the validated k_topk_warp returns (which
-    the tests above pin on the oracle) -- OR with 1..8 clauses incl. absent terms and tails, several k, batches whose
-    large queries are cut into doc-range items and merged, and the signal combine with 4 and 2 columns."""
-    dfs = [1, 5, 127, 128, 129, 300, 1000, 1280, 5000, 20000, 40000, 60000, 90000]
-    (oseg, seg), rng = random_index(31, 200_000, dfs)
+def union_kernel_against_oracle(seed, max_doc, dfs, nq, ks, pad_every, sig_nq, sig_k):
+    """k_or3 against the oracle: OR batches of 1/2/3/5/8 clauses (every `pad_every`-th query of 3+ clauses padded with
+    NO_TERM) whose large queries are cut into doc-range items and merged, compared query by query with the exhaustive
+    union; and the signal combine with 4 / 2 / 0 columns."""
+    (oseg, seg), rng = random_index(seed, max_doc, dfs)
     nt = len(dfs)
-
-    def both(fn):
-        monkeypatch.delenv("SB200_BM25_OR3", raising=False)
-        a = fn()
-        monkeypatch.setenv("SB200_BM25_OR3", "1")
-        b = fn()
-        monkeypatch.delenv("SB200_BM25_OR3", raising=False)
-        return a, b
-
     for width in (1, 2, 3, 5, 8):
-        nq = 120
         terms = np.stack([rng.choice(nt, width, replace=False) for _ in range(nq)]).astype(np.uint32)
         if width >= 3:
-            terms[::7, 1] = NO_TERM   # padded / absent clauses
-        for k in (1, 10, 1000):
-            (ad, as_, an), (bd, bs, bn) = both(lambda: TopDocs.with_limit(k).search_batch(seg, terms, MODE_OR))
-            assert np.array_equal(an, bn), (width, k)
+            terms[::pad_every, 1] = NO_TERM   # padded / absent clauses
+        for k in ks:
+            gd, gs, gn = TopDocs.with_limit(k).search_batch(seg, terms, MODE_OR)
             for q in range(nq):
-                assert np.array_equal(ad[q, :an[q]], bd[q, :bn[q]]) and np.array_equal(as_[q, :an[q]], bs[q, :bn[q]]), (width, k, q)
+                qq = np.array([x for x in terms[q] if x != NO_TERM], np.uint32)
+                w, caches = weights_for(seg, qq)
+                od, os_, _ = oseg.topk(qq, w, caches, 2, k)      # oracle mode 2 = exhaustive union
+                m = int(gn[q])
+                assert m == len(od), (width, k, q, m, len(od))
+                assert np.array_equal(gd[q, :m], od) and np.array_equal(gs[q, :m], os_), (width, k, q)
+    cache = bm25.compute_tf_cache(seg.average_fieldnorm)
     for ncols in (4, 2, 0):
-        cols = [rng.random(200_000) for _ in range(ncols)]
-        comp = SignalComputer(seg, SignalTable(cols) if ncols else None, [2.0, 0.02, 2.0, 0.001][:ncols], coeff_text=0.005)
-        terms = np.stack([rng.choice(nt, 5, replace=False) for _ in range(80)]).astype(np.uint32)
-        (ad, at, an), (bd, bt, bn) = both(lambda: comp.top_docs_batch(terms, 1000))
-        assert np.array_equal(an, bn)
-        for q in range(80):
-            assert np.array_equal(ad[q, :an[q]], bd[q, :bn[q]]) and np.array_equal(at[q, :an[q]], bt[q, :bn[q]]), (ncols, q)
+        cols = [rng.random(max_doc) for _ in range(ncols)]
+        coeffs = [2.0, 0.02, 2.0, 0.001][:ncols]
+        comp = SignalComputer(seg, SignalTable(cols) if ncols else None, coeffs, coeff_text=0.005)
+        terms = np.stack([rng.choice(nt, 5, replace=False) for _ in range(sig_nq)]).astype(np.uint32)
+        w = np.array([[bm25.StractBm25Weight.for_one_term(int(seg.doc_freq[t]), seg.max_doc, seg.average_fieldnorm).weight for t in row]
+                      for row in terms], np.float32)
+        od, ot, on, _ = oseg.signal_topk_batch(terms, w, np.tile(cache, (sig_nq * 5, 1)), 1.2, 0.005, cols, coeffs, sig_k, threads=8)
+        gd, gt, gn = comp.top_docs_batch(terms, sig_k)
+        assert np.array_equal(gn, on), ncols
+        for q in range(sig_nq):
+            assert np.array_equal(gd[q, :gn[q]], od[q, :on[q]]) and np.array_equal(gt[q, :gn[q]], ot[q, :on[q]]), (ncols, q)
+
+
+def test_or3_union_kernel_bit_exact():
+    union_kernel_against_oracle(31, 200_000, [1, 5, 127, 128, 129, 300, 1000, 1280, 5000, 20000, 40000, 60000, 90000],
+                                nq=120, ks=(1, 10, 1000), pad_every=7, sig_nq=80, sig_k=1000)
 
 
 def test_or_wand_replay_matches_block_wand_bit_for_bit():
