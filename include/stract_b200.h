@@ -78,7 +78,7 @@ typedef struct {
   uint64_t n_edges_input;  /* edges handed to create */
   uint64_t n_edges_kept;   /* unique, non-skipped, non-self-loop edges in the CSR (all ranks) */
   uint64_t n_edges_local;  /* ... of which this rank owns (== kept when world_size == 1) */
-  uint64_t row_begin, row_end; /* owned destination rows, in INTERNAL (degree-sorted) order */
+  uint64_t row_begin, row_end; /* always 0 and n_nodes: rows are owned in interleaved 32-row blocks (sb200_graph_ownership) */
   uint64_t hbm_bytes;      /* device memory held by the handle */
   double stage_ms;         /* device time spent in create (relabel + CSR build) */
 } sb200_graph_info;
@@ -152,7 +152,7 @@ SB200_API int sb200_graph_node_ids(sb200_graph* g, uint64_t first, uint64_t coun
  *   frontier  : N-bit changed bitmap; each 32-bit word has a single owner (ownership is in 32-row blocks)
  *               and non-owners hold 0, so the same byte-wise max all-reduce yields the union;
  * then sums the per-rank changed counts and calls sb200_hyperball_exchange_done.
- * sb200_graph_row_ranges is kept for ABI compatibility and returns [0, ..., 0, N] for interleaved handles. */
+ * sb200_graph_row_ranges is kept for ABI compatibility and returns [0, ..., 0, N]. */
 SB200_API int sb200_hyperball_exchange_ptrs(sb200_graph* g, void** regs, uint64_t* regs_bytes,
                                   void** frontier_words, uint64_t* frontier_bytes);
 SB200_API int sb200_graph_row_ranges(sb200_graph* g, uint64_t* begins /* world_size+1 */);
@@ -252,10 +252,11 @@ SB200_API int sb200_inbound_similarity(sb200_graph* g, const uint64_t* liked_lo,
                                        const uint64_t* cand_lo, const uint64_t* cand_hi, uint32_t n_cand, int normalized,
                                        double self_score, double* scores);
 
-/* Tuning switches of one handle (the SB200_* environment variables give the defaults): "quad_side_ctas" (CTAs per SM of the
- * short-row kernel on the side stream of the fused exchange, 0 = one stream), "owned_items" (0 / 1: launch the long-row kernel
- * over the owned work items only), "publish_all" (0 / 1: store produced rows into every peer, no subscriber filter).  All
- * ranks of a sharded computation must use the same "publish_all".  Not while an iteration is in flight. */
+/* Tuning switches of one handle: "quad_side_ctas" (CTAs per SM of the short-row kernel on the side stream of the fused
+ * exchange, 0 = one stream; default 2 with up to 4 ranks or one multicast target, else 0), "owned_items" (0 / 1: launch the
+ * long-row kernel over the owned work items only; default 1), "publish_all" (0 / 1: store produced rows into every peer, no
+ * subscriber filter; default 0).  All ranks of a sharded computation must use the same "publish_all".  Not while an
+ * iteration is in flight. */
 SB200_API int sb200_hyperball_set_option(sb200_graph* g, const char* name, double value);
 
 /* Device-memory arena diagnostics.  With SB200_ARENA=1 in the environment, staging temporaries, the CSR and the

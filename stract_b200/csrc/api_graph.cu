@@ -133,7 +133,7 @@ void sb200_graph_destroy(sb200_graph* g) {
 int sb200_graph_get_info(const sb200_graph* g, sb200_graph_info* info) {
   if (!g || !info) SB_FAIL(SB200_EINVAL, "NULL argument");
   info->n_nodes = g->N; info->n_edges_input = g->E_in; info->n_edges_kept = g->E_kept; info->n_edges_local = g->E_local;
-  info->row_begin = g->row_begin; info->row_end = g->row_end; info->hbm_bytes = g->hbm_bytes(); info->stage_ms = g->stage_ms;
+  info->row_begin = 0; info->row_end = g->N; info->hbm_bytes = g->hbm_bytes(); info->stage_ms = g->stage_ms;
   return SB200_OK;
 }
 
@@ -248,7 +248,7 @@ int sb200_hyperball_exchange_ptrs(sb200_graph* g, void** regs, uint64_t* regs_by
 }
 int sb200_graph_row_ranges(sb200_graph* g, uint64_t* begins) {
   if (!g || !begins) SB_FAIL(SB200_EINVAL, "NULL argument");
-  for (int r = 0; r <= g->world; r++) begins[r] = (g->world > 1) ? (r == g->world ? g->N : 0) : g->range_begins[r];
+  for (int r = 0; r <= g->world; r++) begins[r] = r == g->world ? g->N : 0;
   return SB200_OK;
 }
 // ---- fused exchange over NVLink peer memory (CUDA IPC between the per-GPU processes) ----------------------
@@ -340,7 +340,7 @@ int sb200_hyperball_set_publish_targets(sb200_graph* g, int n_targets, const uin
   g->n_peers = n_targets; g->peers_ipc = false; g->p2p = n_targets > 0;
   // world_size-1 unicast targets are taken in rank order (own rank left out); any other count (e.g. the single
   // multicast mapping) reaches every replica at once, so the subscriber filter is off
-  if (n_targets == g->world - 1) { for (int p = 0; p < n_targets; p++) g->peer_rank[p] = p < g->rank ? p : p + 1; g->publish_all = env_flag("SB200_PUBLISH_ALL", false); }
+  if (n_targets == g->world - 1) { for (int p = 0; p < n_targets; p++) g->peer_rank[p] = p < g->rank ? p : p + 1; g->publish_all = false; }
   else g->publish_all = true;
   return SB200_OK;
 }

@@ -175,17 +175,7 @@ __device__ __forceinline__ bool ne_u4(uint4 a, uint4 b) {
   return ((a.x ^ b.x) | (a.y ^ b.y) | (a.z ^ b.z) | (a.w ^ b.w)) != 0u;
 }
 
-// streaming (read-once) 16-byte load: do not allocate in L1, evict-first in L2
-__device__ __forceinline__ uint4 ld_stream_u4(const uint4* p) {
-#ifndef SB200_EMU
-  uint4 v;
-  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-#else
-  return *p;
-#endif
-}
+// streaming (read-once) load: do not allocate in L1
 __device__ __forceinline__ uint32_t ld_stream_u32(const uint32_t* p) {
 #ifndef SB200_EMU
   uint32_t v;
@@ -193,45 +183,6 @@ __device__ __forceinline__ uint32_t ld_stream_u32(const uint32_t* p) {
   return v;
 #else
   return *p;
-#endif
-}
-
-// L2 eviction hints (experiment switch SB200_L2_HINTS, hyperball.cu): a cache policy made once per thread and passed to
-// the streaming accesses -- source indices, the row being rebuilt, its store -- so that they leave the L2 first and the
-// gathered counter rows (the only data with reuse) stay.  The policy travels in the memory descriptor: no extra
-// instruction per access.
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-#ifndef SB200_EMU
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-#else
-  return 0;
-#endif
-}
-__device__ __forceinline__ uint32_t ld_stream_hint_u32(const uint32_t* a, uint64_t pol) {
-#ifndef SB200_EMU
-  uint32_t v;
-  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(a), "l"(pol));
-  return v;
-#else
-  (void)pol; return *a;
-#endif
-}
-__device__ __forceinline__ uint4 ld_hint_u4(const uint4* a, uint64_t pol) {
-#ifndef SB200_EMU
-  uint4 v;
-  asm volatile("ld.global.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(a), "l"(pol));
-  return v;
-#else
-  (void)pol; return *a;
-#endif
-}
-__device__ __forceinline__ void st_hint_u4(uint4* a, uint4 v, uint64_t pol) {
-#ifndef SB200_EMU
-  asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" :: "l"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
-#else
-  (void)pol; *a = v;
 #endif
 }
 

@@ -32,8 +32,7 @@ struct sb200_graph {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   uint64_t N = 0, E_in = 0, E_kept = 0, E_local = 0;
-  uint64_t row_begin = 0, row_end = 0;  // owned rows (internal order)
-  uint64_t n_pos = 0;                   // rows [0, n_pos) have in-degree > 0 (globally)
+  uint64_t n_pos = 0;  // rows [0, n_pos) have in-degree > 0 (globally)
   bool has_fwd = false;
   int reuse = 0;  // explicit resets: the source-major CSR (push branch) is only built once a handle is reused
   double stage_ms = 0;
@@ -42,12 +41,9 @@ struct sb200_graph {
   sb200::DevBuf<uint32_t> perm, inv;
   sb200::DevBuf<uint32_t> self_bm;  // [N/32] in RANK order: the node has a kept link to itself (not in the CSR: a no-op for HyperBall)
   sb200::DevBuf<uint32_t> row_ptr, col;
-  uint32_t col_base = 0;  // row_ptr values are global; col[] holds [col_base, col_base+E_local)
   sb200::DevBuf<uint32_t> fwd_ptr, fwd_dst;
-  sb200::DevBuf<uint32_t> row_ranges_host_dummy;
-  uint64_t range_begins[65] = {0};
 
-  // pull work partition (owned rows only)
+  // pull work partition (every row; a sharded handle skips the rows it does not own inside the kernels)
   uint64_t warp_row_begin = 0, warp_row_end = 0;  // rows with deg > QUAD_MAX_DEG: warp-per-chunk
   uint64_t quad_row_begin = 0, quad_row_end = 0;  // rows with 0 < deg <= QUAD_MAX_DEG: quad-per-row
   uint64_t n_items = 0;                           // chunks of the warp rows
@@ -82,7 +78,7 @@ struct sb200_graph {
   void* peer_regs[2][sb200::MAX_PEERS] = {{nullptr}};
   void* peer_bm[2][sb200::MAX_PEERS] = {{nullptr}};
   int peer_rank[sb200::MAX_PEERS] = {0};   // rank behind publish target p
-  bool publish_all = false;                // one multicast target / SB200_PUBLISH_ALL=1: no subscriber filtering
+  bool publish_all = false;                // one multicast target / set_option("publish_all"): no subscriber filtering
   sb200::DevBuf<uint32_t> sub_mask;        // [N] subscriber mask per row (internal order), sharded handles only
   uint64_t n_subscribed = 0;               // sum over owned rows of the number of remote subscribers (profile: NVLink rows per dense iteration)
   // device-side inter-rank barrier (sb200_hyperball_run_sharded)
@@ -93,7 +89,7 @@ struct sb200_graph {
   int step_mode = 0;
   double dense_frac = 0.35, push_div = 48.0;  // mode policy (see hb_step)
   int force_mode = -1;
-  uint64_t l2_window_bytes = 0;  // SB200_L2_PERSIST_MB: persisting-L2 access window over the hot prefix of the `old` register array
+  uint64_t l2_window_bytes = 0;  // persisting-L2 access window over the hot prefix of the `old` register array (hb_alloc_state)
 
   // optional per-kernel-family device timing (bench evidence; CUDA events on this handle's stream)
   enum { F_PULL_WARP_DENSE, F_PULL_QUAD_DENSE, F_PULL_WARP_FRONT, F_PULL_QUAD_FRONT, F_PULL_MERGE, F_PUSH, F_FINALIZE,
@@ -104,7 +100,8 @@ struct sb200_graph {
   cudaEvent_t prof_ev[F_COUNT][2] = {{nullptr}};
   // fused exchange: the short-row kernel runs on a second stream beside the long-row kernel (hyperball.cu, launch_pull)
   int sm_count = 0;
-  int opt_side_ctas = -1, opt_owned_list = -1;   // -1: take the environment default at first use (sb200_hyperball_set_option)
+  int opt_side_ctas = -1;    // -1: the default, chosen at first use (sb200_hyperball_set_option)
+  int opt_owned_list = 1;    // k_pull_warp over the owned work items only (sb200_hyperball_set_option)
   cudaStream_t side_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, side_prof[2] = {nullptr, nullptr};
   bool side_prof_used = false;

@@ -9,8 +9,9 @@
 //   2. every edge mapped to (to_rank<<32 | from_rank), stable radix sort, first-of-run keeps the
 //      FIRST occurrence's rel_flags (unique_by semantics), skipped / self-loop edges dropped;
 //   3. nodes relabelled by in-degree (descending) so that rows of equal length are adjacent:
-//      the degree classes of the pull kernels become contiguous row ranges, CSR rebuilt by a
-//      second sort; a source-major CSR is built for the small-frontier (push) branch.
+//      the degree classes of the pull kernels become contiguous row ranges; the rows of the
+//      sorted keys move as blocks to their new place (k_row_permute).  The source-major CSR of the
+//      small-frontier (push) branch is built lazily from the resident one (build_fwd_csr).
 // Radix sorts / scans / selects are CUB device primitives (staging, not the hot loop).
 #include "graph.cuh"
 
@@ -20,7 +21,6 @@
 #include <algorithm>
 #include <ctime>
 #include <cstdlib>
-#include <vector>
 
 namespace sb200 {
 
@@ -47,40 +47,8 @@ __device__ __forceinline__ uint64_t hash128(uint64_t lo, uint64_t hi) {
 }
 #define EMPTY64 0xFFFFFFFFFFFFFFFFull
 
-// flags: [0] overflow, [1] the all-ones id is present (it doubles as the empty sentinel)
-__global__ void k_insert_nodes(const uint64_t* __restrict__ flo, const uint64_t* __restrict__ fhi,
-                               const uint64_t* __restrict__ tlo, const uint64_t* __restrict__ thi,
-                               uint64_t n_edges, ulonglong2* table, uint64_t mask,
-                               unsigned long long* count, unsigned long long max_count, int* flags) {
-  const uint64_t total = 2 * n_edges;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < total;
-       i += (uint64_t)gridDim.x * blockDim.x) {
-    uint64_t lo, hi;
-    if (i < n_edges) { lo = flo[i]; hi = fhi[i]; } else { lo = tlo[i - n_edges]; hi = thi[i - n_edges]; }
-    if (lo == EMPTY64 && hi == EMPTY64) { flags[1] = 1; continue; }
-    if (*(volatile int*)flags) return;
-    const u128 key = ((u128)hi << 64) | lo;
-    uint64_t slot = hash128(lo, hi) & mask;
-    for (uint64_t probe = 0;; probe++) {
-      ulonglong2 cur = table[slot];
-      if (cur.x == lo && cur.y == hi) break;
-      if (cur.x == EMPTY64 || cur.y == EMPTY64) {
-        // empty, being written, or a key with an all-ones half: the CAS result is the truth
-        u128 old = cas128((u128*)&table[slot], ~(u128)0, key);
-        if (old == ~(u128)0) {
-          unsigned long long c = atomicAdd(count, 1ull);
-          if (c + 1 > max_count) flags[0] = 1;
-          break;
-        }
-        if (old == key) break;
-      }
-      slot = (slot + 1) & mask;
-      if (probe > mask) { flags[0] = 1; break; }
-    }
-  }
-}
-
 // inserts one endpoint and returns the table slot that holds it (0xFFFFFFFF for the all-ones id / on overflow)
+// flags: [0] overflow, [1] the all-ones id is present (it doubles as the empty sentinel)
 __device__ __forceinline__ uint32_t insert_slot(ulonglong2* table, uint64_t mask, uint64_t lo, uint64_t hi,
                                                 unsigned long long* count, unsigned long long max_count, int* flags) {
   if (lo == EMPTY64 && hi == EMPTY64) { flags[1] = 1; return 0xFFFFFFFFu; }
@@ -90,6 +58,7 @@ __device__ __forceinline__ uint32_t insert_slot(ulonglong2* table, uint64_t mask
     const ulonglong2 cur = table[slot];
     if (cur.x == lo && cur.y == hi) return (uint32_t)slot;
     if (cur.x == EMPTY64 || cur.y == EMPTY64) {
+      // empty, being written, or a key with an all-ones half: the CAS result is the truth
       const u128 old = cas128((u128*)&table[slot], ~(u128)0, key);
       if (old == ~(u128)0) {
         const unsigned long long c = atomicAdd(count, 1ull);
@@ -124,18 +93,6 @@ __global__ void k_map_slots(const uint32_t* __restrict__ slot_from, const uint32
   keys[i] = ((uint64_t)rt << 32) | rf;
 }
 
-__device__ __forceinline__ uint32_t lookup_rank(const ulonglong2* __restrict__ table,
-                                                const uint32_t* __restrict__ slot_val, uint64_t mask,
-                                                uint64_t lo, uint64_t hi, uint32_t max_rank) {
-  if (lo == EMPTY64 && hi == EMPTY64) return max_rank;
-  uint64_t slot = hash128(lo, hi) & mask;
-  for (;;) {
-    ulonglong2 cur = table[slot];
-    if (cur.x == lo && cur.y == hi) return slot_val[slot];
-    slot = (slot + 1) & mask;
-  }
-}
-
 __global__ void k_compact_keys(const ulonglong2* __restrict__ table, uint64_t cap, uint64_t* out_lo,
                                uint64_t* out_hi, unsigned long long* counter) {
   for (uint64_t base = blockIdx.x * (uint64_t)blockDim.x; base < cap; base += (uint64_t)gridDim.x * blockDim.x) {
@@ -168,19 +125,6 @@ __global__ void k_assign_ranks(const uint64_t* __restrict__ lo, const uint64_t* 
   }
 }
 
-__global__ void k_map_edges(const uint64_t* __restrict__ flo, const uint64_t* __restrict__ fhi,
-                            const uint64_t* __restrict__ tlo, const uint64_t* __restrict__ thi,
-                            const uint64_t* __restrict__ rel, uint64_t n_edges, uint64_t skip_mask,
-                            const ulonglong2* __restrict__ table, const uint32_t* __restrict__ slot_val,
-                            uint64_t mask, uint32_t max_rank, uint64_t* keys, uint8_t* skip) {
-  uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= n_edges) return;
-  uint32_t rf = lookup_rank(table, slot_val, mask, flo[i], fhi[i], max_rank);
-  uint32_t rt = lookup_rank(table, slot_val, mask, tlo[i], thi[i], max_rank);
-  keys[i] = ((uint64_t)rt << 32) | rf;
-  skip[i] = (rel[i] & skip_mask) != 0;
-}
-
 __global__ void k_mark_keep(const uint64_t* __restrict__ keys, const uint8_t* __restrict__ skip, uint64_t n,
                             uint8_t* keep, uint32_t* self_bm) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -204,19 +148,10 @@ __global__ void k_invert(const uint32_t* __restrict__ perm, uint64_t n, uint32_t
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i < n) inv[perm[i]] = (uint32_t)i;
 }
-// keys in rank space (to<<32|from) -> internal space; swap=true builds the source-major key
-__global__ void k_remap(const uint64_t* __restrict__ in, uint64_t n, const uint32_t* __restrict__ inv,
-                        uint64_t* out, bool swap) {
-  uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  uint64_t k = in[i];
-  uint32_t to = inv[k >> 32], from = inv[(uint32_t)k];
-  out[i] = swap ? (((uint64_t)from << 32) | to) : (((uint64_t)to << 32) | from);
-}
 // Relabelling permutes whole CSR rows: the rank-space keys are already grouped by destination, so row `to` (edges
 // [rank_ptr[to], rank_ptr[to+1])) moves as a block to row_ptr[inv[to]] and only the source ids are translated.
-// One pass instead of a second 64-bit radix sort of all edges (SB200_STAGE_ROWPERM=1).  Sources inside a row stay
-// in rank order instead of internal-id order; the pull kernels take a max over them, so the order is immaterial.
+// One pass instead of a second 64-bit radix sort of all edges.  Sources inside a row stay in rank order instead of
+// internal-id order; the pull kernels take a max over them, so the order is immaterial.
 __global__ void k_row_permute(const uint64_t* __restrict__ keys, uint64_t n, const uint32_t* __restrict__ rank_ptr,
                               const uint32_t* __restrict__ inv, const uint32_t* __restrict__ row_ptr, uint32_t* col) {
   const uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -239,27 +174,6 @@ __global__ void k_class_bounds(const uint32_t* __restrict__ deg, uint64_t n, uin
   if (d > t0 && !(nx > t0)) out[0] = i + 1;
   if (d > t1 && !(nx > t1)) out[1] = i + 1;
   if (d > t2 && !(nx > t2)) out[2] = i + 1;
-}
-// first row whose row_ptr >= target (rows are edge-balanced between ranks), 32-row aligned
-// Rank boundaries by estimated iteration time rather than raw edge count: 68 B per in-edge, 34 B more per in-edge of a
-// quad-per-row row (that kernel moves its bytes more slowly than the warp-per-item one), and ~200 B of row/finalize
-// traffic per row with in-edges: cost(row) = 68*E_before + 34*E_quad_before + 200*min(row, n_pos).
-__device__ __forceinline__ double split_cost(const uint32_t* row_ptr, uint64_t row, uint64_t n_warp, uint64_t n_pos) {
-  const double e = (double)row_ptr[row];
-  const double eq = row > n_warp ? e - (double)row_ptr[n_warp] : 0.0;
-  return 68.0 * e + 34.0 * eq + 200.0 * (double)(row < n_pos ? row : n_pos);
-}
-__global__ void k_find_splits(const uint32_t* __restrict__ row_ptr, uint64_t n, uint64_t E, int world,
-                              const unsigned long long* __restrict__ cls /* [0]=n_pos [1]=n_warp */, unsigned long long* out) {
-  int r = threadIdx.x;
-  if (r > world) return;
-  if (r == 0) { out[0] = 0; return; }
-  if (r == world) { out[r] = n; return; }
-  const uint64_t n_pos = cls[0], n_warp = cls[1];
-  const double target = split_cost(row_ptr, n, n_warp, n_pos) * (double)r / (double)world;
-  uint64_t lo = 0, hi = n;
-  while (lo < hi) { uint64_t mid = (lo + hi) / 2; if (split_cost(row_ptr, mid, n_warp, n_pos) < target) lo = mid + 1; else hi = mid; }
-  out[r] = (lo / 32) * 32;
 }
 __global__ void k_owned_edges(const uint32_t* __restrict__ row_ptr, uint64_t n, uint32_t world, uint32_t rank,
                               unsigned long long* out) {
@@ -542,8 +456,7 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
   SB_TRY(g->row_ptr.alloc(N + 1));
   if (N == 0) {
     SB_CUDA(cudaMemsetAsync(g->row_ptr.p, 0, sizeof(uint32_t), s));
-    g->E_kept = g->E_local = 0; g->row_begin = g->row_end = 0; g->n_pos = 0;
-    for (int r = 0; r <= g->world; r++) g->range_begins[r] = 0;
+    g->E_kept = g->E_local = 0; g->n_pos = 0;
     SB_CUDA(cudaEventRecord(g->ev1, s)); SB_CUDA(cudaStreamSynchronize(s));
     return SB200_OK;
   }
@@ -608,7 +521,7 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
   skip_a.release(); skip_b.release();
 
   pt.mark("3a degrees + node sort");
-  // ---- 3. degree-sorted relabel + CSR (both directions) ------------------------------------------
+  // ---- 3. degree-sorted relabel + destination-major CSR ------------------------------------------
   DevBuf<uint32_t> deg_a, deg_b, val_b; SB_TRY(deg_a.alloc(N)); SB_TRY(deg_b.alloc(N)); SB_TRY(val_b.alloc(N));
   SB_CUDA(cudaMemsetAsync(deg_a.p, 0, N * 4, s));
   if (E) { SB_LAUNCH(k_degree_hi, div_up(E, TPB), TPB, 0, s, k, E, deg_a.p); SB_CHECK_LAUNCH(); }
@@ -625,60 +538,19 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
     SB_CUDA(cudaMemsetAsync(ctr.p, 0, 8 * sizeof(unsigned long long), s));
     SB_LAUNCH(k_class_bounds, div_up(N, TPB), TPB, 0, s, dk, N, 0u, (uint32_t)QUAD_MAX_DEG, (uint32_t)CHUNK_EDGES, ctr.p);
     SB_CHECK_LAUNCH();
+    SB_CUDA(cudaMemcpyAsync(h_ctr, ctr.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     SB_CUDA(cudaStreamSynchronize(s));
   }
-  DevBuf<unsigned long long> splits; SB_TRY(splits.alloc(g->world + 1));
-  SB_LAUNCH(k_find_splits, 1, 128, 0, s, g->row_ptr.p, N, E, g->world, ctr.p, splits.p); SB_CHECK_LAUNCH();
-  std::vector<unsigned long long> h_splits(g->world + 1);
-  SB_CUDA(cudaMemcpyAsync(h_ctr, ctr.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-  SB_CUDA(cudaMemcpyAsync(h_splits.data(), splits.p, (g->world + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-  SB_CUDA(cudaStreamSynchronize(s));
   const uint64_t n_pos = h_ctr[0], n_warp = h_ctr[1], n_multi = h_ctr[2];
   g->n_pos = n_pos;
-  for (int r = 0; r <= g->world; r++) {
-    g->range_begins[r] = h_splits[r];
-    if (r > 0 && g->range_begins[r] < g->range_begins[r - 1]) g->range_begins[r] = g->range_begins[r - 1];
-  }
-  g->range_begins[g->world] = N;
-  g->row_begin = g->range_begins[g->rank];
-  g->row_end = g->range_begins[g->rank + 1];
 
-  pt.mark("3b remap + sort (dst CSR)");
-  // destination-major CSR in internal ids
+  pt.mark("3b row permute (dst CSR)");
+  // destination-major CSR in internal ids: the rows move as blocks instead of re-sorting every edge (see k_row_permute)
   DevBuf<uint32_t> col_full; SB_TRY(col_full.alloc(E));
-  if (E && env_flag("SB200_STAGE_ROWPERM", true) && !(g->world == 1 && getenv("SB200_EAGER_FWD") != nullptr)) {
-    // move the rows as blocks instead of re-sorting every edge (see k_row_permute); SB200_STAGE_ROWPERM=0: second radix sort
+  if (E) {
     DevBuf<uint32_t> rank_ptr; SB_TRY(rank_ptr.alloc(N + 1));
     SB_LAUNCH(k_offsets_from_sorted, div_up(E + 1, TPB), TPB, 0, s, k, E, N, rank_ptr.p); SB_CHECK_LAUNCH();
     SB_LAUNCH(k_row_permute, div_up(E, TPB), TPB, 0, s, k, E, rank_ptr.p, g->inv.p, g->row_ptr.p, col_full.p); SB_CHECK_LAUNCH();
-    pt.mark("3c remap + sort (fwd CSR)");
-    SB_CUDA(cudaStreamSynchronize(s));
-  } else if (E) {
-    SB_LAUNCH(k_remap, div_up(E, TPB), TPB, 0, s, k, E, g->inv.p, k_alt, false); SB_CHECK_LAUNCH();
-    uint64_t *a = k_alt, *b = k;  // sort a (clobbers b = rank-space keys, rebuilt below when needed)
-    // keep the rank-space keys: we need them again for the forward CSR, so sort into a third buffer
-    DevBuf<uint64_t> keys_c; SB_TRY(keys_c.alloc(E));
-    uint64_t* c = keys_c.p;
-    SB_TRY(sort_keys<uint64_t>(tmp, a, c, E, 0, 32 + nb, s));
-    SB_LAUNCH(k_lo32, div_up(E, TPB), TPB, 0, s, a, E, col_full.p); SB_CHECK_LAUNCH();
-    pt.mark("3c remap + sort (fwd CSR)");
-    // source-major CSR (single-rank handles only: the push branch needs every out-edge).  It costs a third sort of all
-    // edges and saves only the tail iterations of a run, so by default it is built lazily by build_fwd_csr() the first
-    // time a REUSED handle meets a small frontier; SB200_EAGER_FWD=1 builds it here.
-    if (g->world == 1 && getenv("SB200_EAGER_FWD") != nullptr) {
-      uint64_t* other = c;  // scratch half of the last sort
-      SB_LAUNCH(k_remap, div_up(E, TPB), TPB, 0, s, b, E, g->inv.p, a, true); SB_CHECK_LAUNCH();
-      SB_TRY(sort_keys<uint64_t>(tmp, a, other, E, 0, 32 + nb, s));
-      SB_TRY(g->fwd_dst.alloc(E)); SB_TRY(g->fwd_ptr.alloc(N + 1));
-      SB_LAUNCH(k_lo32, div_up(E, TPB), TPB, 0, s, a, E, g->fwd_dst.p); SB_CHECK_LAUNCH();
-      SB_CUDA(cudaMemsetAsync(deg_b.p == dk ? deg_a.p : deg_b.p, 0, N * 4, s));
-      uint32_t* od = (deg_b.p == dk) ? deg_a.p : deg_b.p;
-      SB_LAUNCH(k_degree_hi, div_up(E, TPB), TPB, 0, s, a, E, od); SB_CHECK_LAUNCH();
-      SB_TRY(exclusive_scan_u32(tmp, od, g->fwd_ptr.p, N, s));
-      uint32_t e32 = (uint32_t)E;
-      SB_CUDA(cudaMemcpyAsync(g->fwd_ptr.p + N, &e32, 4, cudaMemcpyHostToDevice, s));
-      g->has_fwd = true;
-    }
     SB_CUDA(cudaStreamSynchronize(s));
   } else if (g->world == 1) {
     SB_TRY(g->fwd_ptr.alloc(N + 1));
@@ -694,8 +566,6 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
   // which balances both the gather work and -- decisive on 8 GPUs -- the bytes each rank has to push to its peers
   // (a contiguous edge-balanced split left one rank owning 78 % of the rows and 9.7 GB of NVLink egress per
   // iteration).  Every rank keeps the full CSR and filters by ownership inside the kernels.
-  if (g->world > 1) { g->row_begin = 0; g->row_end = N; }
-  g->col_base = 0;
   g->E_local = E;
   g->col = std::move(col_full);
   if (g->world > 1 && N) {
@@ -706,9 +576,8 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
     SB_CUDA(cudaStreamSynchronize(s));
     g->E_local = h_ctr[0];
   }
-  auto clampr = [&](uint64_t x) { return std::min(std::max(x, g->row_begin), g->row_end); };
-  g->warp_row_begin = clampr(0); g->warp_row_end = clampr(n_warp);
-  g->quad_row_begin = clampr(n_warp); g->quad_row_end = clampr(n_pos);
+  g->warp_row_begin = 0; g->warp_row_end = n_warp;
+  g->quad_row_begin = n_warp; g->quad_row_end = n_pos;
   {
     uint32_t rp[3] = {0, 0, 0};
     SB_CUDA(cudaMemcpyAsync(&rp[0], g->row_ptr.p + g->warp_row_begin, 4, cudaMemcpyDeviceToHost, s));
@@ -730,11 +599,10 @@ int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi
     SB_TRY(g->item_start.alloc(nwr + 1));
     SB_TRY(exclusive_scan_u32(tmp, nchunks.p, g->item_start.p, nwr + 1, s));
     uint32_t total = 0, multi_items = 0;
-    const uint64_t nmr = (clampr(n_multi) > g->warp_row_begin) ? clampr(n_multi) - g->warp_row_begin : 0;
     SB_CUDA(cudaMemcpyAsync(&total, g->item_start.p + nwr, 4, cudaMemcpyDeviceToHost, s));
-    SB_CUDA(cudaMemcpyAsync(&multi_items, g->item_start.p + nmr, 4, cudaMemcpyDeviceToHost, s));
+    SB_CUDA(cudaMemcpyAsync(&multi_items, g->item_start.p + n_multi, 4, cudaMemcpyDeviceToHost, s));
     SB_CUDA(cudaStreamSynchronize(s));
-    g->n_items = total; g->n_multi_rows = nmr; g->n_multi_items = multi_items;
+    g->n_items = total; g->n_multi_rows = n_multi; g->n_multi_items = multi_items;
     SB_TRY(g->item_row.alloc(total));
     SB_LAUNCH(k_fill_items, div_up(total, TPB), TPB, 0, s, g->item_start.p, nwr, (uint64_t)total,
               (uint32_t)g->warp_row_begin, g->item_row.p);

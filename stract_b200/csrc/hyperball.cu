@@ -205,11 +205,11 @@ __device__ __forceinline__ bool bm_test(const uint32_t* __restrict__ bm, uint32_
 // the sources are built from seed[] (2 B per source, L2-resident) and `oldr` is not read.
 template <bool FRONTIER, bool SEED>
 __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub, uint32_t lane,
-    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
+    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut& peers) {
   static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
-  const uint32_t e0 = live ? row_ptr[row] - col_base : 0u, e1 = live ? row_ptr[row + 1] - col_base : 0u;
+  const uint32_t e0 = live ? row_ptr[row] : 0u, e1 = live ? row_ptr[row + 1] : 0u;
   const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub) : oldr[row * 4 + sub];
   uint4 acc = own;
   // lane `sub` fetches source index e+sub (one 16-B request per quad per 4 edges, prefetched one step ahead)
@@ -257,7 +257,7 @@ __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub,
 
 template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64_t row_end,
-    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
+    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
   const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -268,7 +268,7 @@ __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64
   if (!live) row = row_end - 1;  // keep the warp converged; results of dead quads are discarded
   live = live && owned_row(peers, (uint32_t)row);
   if (__ballot_sync(0xffffffffu, live) == 0u) return;  // none of this warp's rows belongs to this rank
-  quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, col_base, oldr, seed, newr, bm_prev, bm_cur, peers);
+  quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers);
 }
 
 // Sharded handles with the fused exchange: the short rows are most of the rows, so this kernel carries most of the
@@ -277,7 +277,7 @@ __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64
 // sit next to k_pull_warp on a second, higher-priority stream: link traffic of the short rows under the gathers of the long ones.
 template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, uint64_t row_end, uint64_t first_block, uint64_t n_tasks,
-    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
+    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
   const uint32_t sub = threadIdx.x & 3, lane = threadIdx.x & 31;
@@ -288,54 +288,8 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, 
     const bool live = row >= row_begin && row < row_end;
     if (!live) row = row_begin;
     if (__ballot_sync(0xffffffffu, live) == 0u) continue;
-    quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, col_base, oldr, seed, newr, bm_prev, bm_cur, peers);
+    quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers);
   }
-}
-
-// Experiment (SB200_QUAD2=1, single-rank handles): two adjacent rows per quad, their index loads and gathers interleaved --
-// twice the loads in flight per lane for the short-row class, whose gathers wait on DRAM latency.  40 registers => 6
-// CTAs/SM instead of 7.
-template <bool FRONTIER>
-__global__ void __launch_bounds__(256, 4) k_pull_quad2(uint64_t row_begin, uint64_t row_end,
-    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
-    const uint4* __restrict__ oldr, uint4* __restrict__ newr,
-    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur) {
-  const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  const uint32_t sub = threadIdx.x & 3, lane = threadIdx.x & 31;
-  const uint64_t pair = gt >> 2;
-  uint64_t rowA = row_begin + 2 * pair, rowB = rowA + 1;
-  const bool liveA = rowA < row_end, liveB = rowB < row_end;
-  if (!liveA) rowA = row_end - 1;
-  if (!liveB) rowB = row_end - 1;
-  if (__ballot_sync(0xffffffffu, liveA) == 0u) return;
-  const uint32_t a0 = liveA ? row_ptr[rowA] : 0u, a1 = liveA ? row_ptr[rowA + 1] : 0u;
-  const uint32_t b0 = liveB ? row_ptr[rowB] : 0u, b1 = liveB ? row_ptr[rowB + 1] : 0u;
-  uint4 accA = oldr[rowA * 4 + sub], accB = oldr[rowB * 4 + sub];
-  const unsigned qmask = 0xFu << (lane & ~3u);
-  const uint32_t selfA = (uint32_t)rowA, selfB = (uint32_t)rowB;
-  const uint32_t steps = max((a1 - a0 + 3u) >> 2, (b1 - b0 + 3u) >> 2);
-  uint32_t nA = (a0 + sub < a1) ? ld_stream_u32(col + a0 + sub) : selfA;
-  uint32_t nB = (b0 + sub < b1) ? ld_stream_u32(col + b0 + sub) : selfB;
-  for (uint32_t i = 0; i < steps; i++) {
-    uint32_t mA = nA, mB = nB;
-    const uint32_t ea = a0 + 4 * (i + 1) + sub, eb = b0 + 4 * (i + 1) + sub;
-    nA = (ea < a1) ? ld_stream_u32(col + ea) : selfA;
-    nB = (eb < b1) ? ld_stream_u32(col + eb) : selfB;
-    if (FRONTIER) { mA = bm_test(bm_prev, mA) ? mA : selfA; mB = bm_test(bm_prev, mB) ? mB : selfB; }
-    const uint32_t iA0 = __shfl_sync(qmask, mA, 0, 4), iA1 = __shfl_sync(qmask, mA, 1, 4), iA2 = __shfl_sync(qmask, mA, 2, 4), iA3 = __shfl_sync(qmask, mA, 3, 4);
-    const uint32_t iB0 = __shfl_sync(qmask, mB, 0, 4), iB1 = __shfl_sync(qmask, mB, 1, 4), iB2 = __shfl_sync(qmask, mB, 2, 4), iB3 = __shfl_sync(qmask, mB, 3, 4);
-    const uint4 vA0 = oldr[(uint64_t)iA0 * 4 + sub], vA1 = oldr[(uint64_t)iA1 * 4 + sub], vA2 = oldr[(uint64_t)iA2 * 4 + sub], vA3 = oldr[(uint64_t)iA3 * 4 + sub];
-    const uint4 vB0 = oldr[(uint64_t)iB0 * 4 + sub], vB1 = oldr[(uint64_t)iB1 * 4 + sub], vB2 = oldr[(uint64_t)iB2 * 4 + sub], vB3 = oldr[(uint64_t)iB3 * 4 + sub];
-    accA = vmax_u8x16(vmax_u8x16(accA, vA0), vmax_u8x16(vmax_u8x16(vA1, vA2), vA3));
-    accB = vmax_u8x16(vmax_u8x16(accB, vB0), vmax_u8x16(vmax_u8x16(vB1, vB2), vB3));
-  }
-  const uint4 ownA = oldr[rowA * 4 + sub], ownB = oldr[rowB * 4 + sub];   // re-read (L1/L2 hit) instead of holding 8 registers across the loop
-  const unsigned ballA = __ballot_sync(0xffffffffu, ne_u4(accA, ownA)), ballB = __ballot_sync(0xffffffffu, ne_u4(accB, ownB));
-  const bool chA = ((ballA >> (lane & ~3u)) & 0xFu) != 0u, chB = ((ballB >> (lane & ~3u)) & 0xFu) != 0u;
-  if (liveA && (chA || bm_test(bm_prev, selfA))) newr[rowA * 4 + sub] = accA;
-  if (liveA && chA && sub == 0) atomicOr(bm_cur + (selfA >> 5), 1u << (selfA & 31));
-  if (liveB && (chB || bm_test(bm_prev, selfB))) newr[rowB * 4 + sub] = accB;
-  if (liveB && chB && sub == 0) atomicOr(bm_cur + (selfB >> 5), 1u << (selfB & 31));
 }
 
 // ---- pull, long rows: one warp per <=CHUNK_EDGES work item ---------------------------------------------
@@ -344,7 +298,7 @@ template <bool FRONTIER, bool LISTED, bool SEED>
 // number of resident warps
 __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t first_multi_free_item,
     const uint32_t* __restrict__ item_list, const uint32_t* __restrict__ item_row, const uint32_t* __restrict__ item_start, uint32_t warp_row_begin,
-    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col, uint32_t col_base,
+    const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr, uint4* __restrict__ partial,
     const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
   static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
@@ -355,7 +309,7 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
   const uint32_t row = item_row[item];
   if (!owned_row(peers, row)) return;  // sharded: another rank owns this row (warp-uniform)
   const uint32_t chunk = (uint32_t)item - item_start[row - warp_row_begin];
-  const uint32_t rs = row_ptr[row] - col_base, re = row_ptr[row + 1] - col_base;
+  const uint32_t rs = row_ptr[row], re = row_ptr[row + 1];
   const uint32_t e0 = rs + chunk * (uint32_t)CHUNK_EDGES;
   const uint32_t e1 = min(e0 + (uint32_t)CHUNK_EDGES, re);
   uint4 acc = make_uint4(0, 0, 0, 0);
@@ -693,15 +647,17 @@ __global__ void k_gather_f64x2(const uint32_t* __restrict__ inv, const double* _
   oa[i] = a[v]; ob[i] = b[v];
 }
 
-static double env_f(const char* name, double dflt) {
-  const char* s = getenv(name);
-  return s ? atof(s) : dflt;
-}
+// Rows are ordered by in-degree, so the head of the register array holds the hubs -- on a power-law graph also the
+// most-gathered sources.  The first L2_WINDOW_BYTES of the array being READ are pinned as persisting L2 lines for the pull
+// kernels (stream access-policy window, re-pointed at the `old` array every iteration), so the streaming col/row traffic
+// cannot evict them.
+// H100 80 GB at 400 W, C2 (25 M ids / 500 M edges): 0 -> 53.6, 16 -> 47.9, 32 -> 67.0 ms/step (32 of the 50 MB L2 starve the streams)
+// The seed iteration (t = 0) points the window at the seed array instead, capped at the same size.  Iteration 0 of C2
+// (28.8 MB of seeds), same card: no window 6.87, 16 MB 6.93, the whole array (a 30 MB window) 6.18 ms -- but a
+// 30 MB set-aside slows the dense iterations from 8.4 to 10.3 ms, so the cap stays.
+constexpr uint64_t L2_WINDOW_BYTES = 16ull << 20;
 
 int hb_alloc_state(sb200_graph* g) {
-  g->dense_frac = env_f("SB200_DENSE_FRAC", g->dense_frac);
-  g->push_div = env_f("SB200_PUSH_DIV", g->push_div);
-  g->force_mode = (int)env_f("SB200_FORCE_MODE", (double)g->force_mode);
   const uint64_t N = g->N;
   const uint64_t words = (N + 31) / 32;
   SB_TRY(load_tables(g->device));
@@ -715,28 +671,16 @@ int hb_alloc_state(sb200_graph* g) {
   if (g->world > 1) {   // sync page of the device-side barrier (plain cudaMalloc: exported through CUDA IPC)
     SB_TRY(g->sync_page.alloc(SYNC_SLOTS));
     SB_CUDA(cudaMemset(g->sync_page.p, 0, SYNC_SLOTS * sizeof(unsigned long long)));
-    g->publish_all = env_flag("SB200_PUBLISH_ALL", false);
   }
   if (!g->h_counters) SB_CUDA(cudaMallocHost((void**)&g->h_counters, 8 * sizeof(unsigned long long)));
-  // Rows are ordered by in-degree, so the head of the register array holds the hubs -- on a power-law graph also the
-  // most-gathered sources.  The first SB200_L2_PERSIST_MB (default 16; 0 = off) MB of the array being READ are pinned
-  // as persisting L2 lines for the pull kernels (stream access-policy window, re-pointed at the `old` array every
-  // iteration), so the streaming col/row traffic cannot evict them.
-  // H100 80 GB at 400 W, C2 (25 M ids / 500 M edges): 0 -> 53.6, 16 -> 47.9, 32 -> 67.0 ms/step (32 of the 50 MB L2 starve the streams)
-  // The seed iteration (t = 0) points the window at the seed array instead, capped at the same size.  Iteration 0 of C2
-  // (28.8 MB of seeds), same card: no window 6.87, 16 MB 6.93, the whole array (SB200_L2_PERSIST_MB=30) 6.18 ms -- but a
-  // 30 MB set-aside slows the dense iterations from 8.4 to 10.3 ms, so the cap stays.
-  const double mb = env_f("SB200_L2_PERSIST_MB", 16.0);
+  cudaDeviceProp prop;
+  SB_CUDA(cudaGetDeviceProperties(&prop, g->device));
+  uint64_t want = L2_WINDOW_BYTES;
+  want = std::min<uint64_t>(want, (uint64_t)std::max(prop.persistingL2CacheMaxSize, 0));
+  want = std::min<uint64_t>(want, (uint64_t)std::max(prop.accessPolicyMaxWindowSize, 0));
+  want = std::min<uint64_t>(want, N * 64);
   g->l2_window_bytes = 0;
-  if (mb > 0) {
-    cudaDeviceProp prop;
-    SB_CUDA(cudaGetDeviceProperties(&prop, g->device));
-    uint64_t want = (uint64_t)(mb * 1048576.0);
-    want = std::min<uint64_t>(want, (uint64_t)std::max(prop.persistingL2CacheMaxSize, 0));
-    want = std::min<uint64_t>(want, (uint64_t)std::max(prop.accessPolicyMaxWindowSize, 0));
-    want = std::min<uint64_t>(want, N * 64);
-    if (want) { SB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want)); g->l2_window_bytes = want; }
-  }
+  if (want) { SB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want)); g->l2_window_bytes = want; }
   return SB200_OK;
 }
 
@@ -803,9 +747,10 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
   // fused exchange: short rows on the side stream, next to the long-row kernel (see k_pull_quad_owned)
   if (g->opt_side_ctas < 0) {
     // default: the side stream for up to 4 ranks and for one multicast target; with unicast stores to 7 peers the short-row
-    // kernel beside the long-row one slows both (not measured on H100: it needs several GPUs; SB200_QUAD_SIDE_CTAS overrides)
+    // kernel beside the long-row one slows both (not measured on H100: it needs several GPUs; set_option("quad_side_ctas")
+    // overrides)
     const bool multicast_target = g->n_peers < g->world - 1;
-    g->opt_side_ctas = (int)env_f("SB200_QUAD_SIDE_CTAS", (multicast_target || g->world <= 4) ? 2.0 : 0.0);
+    g->opt_side_ctas = (multicast_target || g->world <= 4) ? 2 : 0;
   }
   const int side_ctas = g->opt_side_ctas;
   const bool side_quad = side_ctas > 0 && g->world > 1 && g->p2p && g->n_peers > 0 && g->n_items && g->quad_row_end > g->quad_row_begin;
@@ -831,12 +776,11 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
       SB_TRY(set_l2_window(g->side_stream, wbase, wbytes));
     }
     if (g->profiling) SB_CUDA(cudaEventRecord(g->side_prof[0], g->side_stream));
-    if (getenv("SB200_DEBUG_SIDE")) fprintf(stderr, "[sb200] side quad: rank %d tasks %llu\n", g->rank, (unsigned long long)n_tasks);
     if (n_tasks) {
       const unsigned grid = (unsigned)std::min<uint64_t>(div_up(n_tasks, 8), (uint64_t)sm_count * (uint64_t)side_ctas);
       auto kern = k_pull_quad_owned<FRONTIER, SEED>;
       SB_LAUNCH(kern, grid, 256, 0, g->side_stream, g->quad_row_begin, g->quad_row_end, first, n_tasks,
-                g->row_ptr.p, g->col.p, g->col_base, oldr, g->seed.p, newr, bmp, bmc, po);
+                g->row_ptr.p, g->col.p, oldr, g->seed.p, newr, bmp, bmc, po);
       SB_CHECK_LAUNCH();
     }
     if (g->profiling) {
@@ -847,13 +791,12 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
   }
   if (g->n_items) {
     PROF_BEGIN(g, FW);
-    if (g->opt_owned_list < 0) g->opt_owned_list = env_flag("SB200_OWNED_ITEMS", true) ? 1 : 0;
     const bool listed = g->opt_owned_list > 0 && g->world > 1 && g->owned_items.p;
     const uint64_t n_launch = listed ? g->n_owned_items : g->n_items;
     auto kern = listed ? k_pull_warp<FRONTIER, true, SEED> : k_pull_warp<FRONTIER, false, SEED>;
     if (n_launch)
     SB_LAUNCH(kern, div_up(n_launch * 32, 256), 256, 0, s, n_launch, g->n_multi_items,
-              listed ? g->owned_items.p : (const uint32_t*)nullptr, g->item_row.p, g->item_start.p, (uint32_t)g->warp_row_begin, g->row_ptr.p, g->col.p, g->col_base, oldr,
+              listed ? g->owned_items.p : (const uint32_t*)nullptr, g->item_row.p, g->item_start.p, (uint32_t)g->warp_row_begin, g->row_ptr.p, g->col.p, oldr,
               g->seed.p, newr, g->partial.p, bmp, bmc, po);
     SB_CHECK_LAUNCH();
     PROF_END(g, FW, g->own_frac * (per_edge * (double)g->E_warp + 68.0 * (double)(g->warp_row_end - g->warp_row_begin - g->n_multi_rows)));
@@ -869,14 +812,9 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
   if (side_quad) { SB_CUDA(cudaEventRecord(g->ev_join, g->side_stream)); SB_CUDA(cudaStreamWaitEvent(s, g->ev_join, 0)); }
   else if (nq) {
     PROF_BEGIN(g, FQ);
-    static const bool quad2 = env_flag("SB200_QUAD2", false);
     auto kern = k_pull_quad<FRONTIER, SEED>;
-    if (quad2 && !SEED && g->world == 1 && g->col_base == 0)
-      SB_LAUNCH(k_pull_quad2<FRONTIER>, div_up(((nq + 1) / 2) * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
-                g->col.p, oldr, newr, bmp, bmc);
-    else
     SB_LAUNCH(kern, div_up(nq * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
-              g->col.p, g->col_base, oldr, g->seed.p, newr, bmp, bmc, po);
+              g->col.p, oldr, g->seed.p, newr, bmp, bmc, po);
     SB_CHECK_LAUNCH();
     PROF_END(g, FQ, g->own_frac * (per_edge * (double)g->E_quad + 68.0 * (double)nq));
   }
@@ -1083,13 +1021,12 @@ int hb_step_launch(sb200_graph* g, bool with_barrier) {
     }
   } else {
     // sharded handles: the same lazy rule for the source-major CSR (of the owned rows); every rank sees the same
-    // global changed count, so all ranks switch together (SB200_SHARDED_PUSH=0 keeps them on the pull kernels)
+    // global changed count, so all ranks switch together
     // Thresholds: below 0.75 N changed nodes a frontier-filtered pull reads fewer source registers than a dense one (the
     // rule of a single rank without forward CSR); below N / 16 a push over the changed rows' out-edges does less work than a
     // frontier pull, which still scans every local edge.
-    static const bool auto_push = env_flag("SB200_SHARDED_PUSH", true);
     const bool tiny = (double)g->n_changed_prev * 16.0 <= (double)N;
-    if (!g->has_fwd && ((auto_push && g->reuse > 0 && g->t > 0 && tiny) || force_mode == 2)) SB_TRY(build_fwd_csr(g));
+    if (!g->has_fwd && ((g->reuse > 0 && g->t > 0 && tiny) || force_mode == 2)) SB_TRY(build_fwd_csr(g));
     if (g->has_fwd && tiny) mode = 2;
     else mode = ((double)g->n_changed_prev >= 0.75 * (double)N) ? 0 : 1;
   }
@@ -1119,17 +1056,14 @@ int hb_step_launch(sb200_graph* g, bool with_barrier) {
     SB_LAUNCH(k_publish_bitmap, div_up(words, 256), 256, 0, s, bmc, words, po);
     SB_CHECK_LAUNCH();
   }
-  const uint64_t nrows = g->row_end - g->row_begin;
-  if (nrows) {
-    PROF_BEGIN(g, sb200_graph::F_FINALIZE);
-    if (!g->sm_count) SB_CUDA(cudaDeviceGetAttribute(&g->sm_count, cudaDevAttrMultiProcessorCount, g->device));
-    const unsigned fin_grid = (unsigned)std::min<uint64_t>(div_up(div_up(nrows, (uint64_t)std::max(g->world, 1)), 256) + 1, (uint64_t)g->sm_count * 8);
-    SB_LAUNCH(k_finalize, fin_grid, 256, 0, s, g->row_begin, g->row_end, newr, bmp, bmc, g->size_cache.p,
-              g->kahan_sum.p, g->kahan_err.p, g->has_fwd ? g->fwd_ptr.p : (const uint32_t*)nullptr, (double)(g->t + 1),
-              g->counters.p, (uint32_t)g->world, (uint32_t)g->rank);
-    SB_CHECK_LAUNCH();
-    PROF_END(g, sb200_graph::F_FINALIZE, 0.25 * (double)nrows);  // 2 bitmap bits/row; + 112 B per changed row below
-  }
+  PROF_BEGIN(g, sb200_graph::F_FINALIZE);
+  if (!g->sm_count) SB_CUDA(cudaDeviceGetAttribute(&g->sm_count, cudaDevAttrMultiProcessorCount, g->device));
+  const unsigned fin_grid = (unsigned)std::min<uint64_t>(div_up(div_up(N, (uint64_t)std::max(g->world, 1)), 256) + 1, (uint64_t)g->sm_count * 8);
+  SB_LAUNCH(k_finalize, fin_grid, 256, 0, s, (uint64_t)0, N, newr, bmp, bmc, g->size_cache.p,
+            g->kahan_sum.p, g->kahan_err.p, g->has_fwd ? g->fwd_ptr.p : (const uint32_t*)nullptr, (double)(g->t + 1),
+            g->counters.p, (uint32_t)g->world, (uint32_t)g->rank);
+  SB_CHECK_LAUNCH();
+  PROF_END(g, sb200_graph::F_FINALIZE, 0.25 * (double)N);  // 2 bitmap bits/row; + 112 B per changed row below
   if (g->p2p) SB_CUDA(cudaMemsetAsync((void*)bmp, 0, (words + 1) * 4, s));  // next step's `cur` bitmap
   if (with_barrier) {
     if (!g->sync_page.p || g->n_peers != g->world - 1) SB_FAIL(SB200_ESTATE, "device barrier needs the sync pages of all %d peers", g->world - 1);
@@ -1202,7 +1136,7 @@ int hb_result(sb200_graph* g, uint64_t* id_lo, uint64_t* id_hi, double* cent, ui
   SB_TRY(flag.alloc(N + 1)); SB_TRY(pos.alloc(N + 1)); SB_TRY(val.alloc(N));
   SB_CUDA(cudaMemsetAsync(flag.p + N, 0, 4, s));
   const double norm = (double)(N - 1);
-  SB_LAUNCH(k_result_flags, div_up(N, 256), 256, 0, s, g->inv.p, g->kahan_sum.p, N, g->row_begin, g->row_end, norm, flag.p, val.p,
+  SB_LAUNCH(k_result_flags, div_up(N, 256), 256, 0, s, g->inv.p, g->kahan_sum.p, N, (uint64_t)0, N, norm, flag.p, val.p,
             (uint32_t)g->world, (uint32_t)g->rank);
   SB_CHECK_LAUNCH();
   size_t need = 0;
@@ -1263,7 +1197,7 @@ int hb_ranked(sb200_graph* g, int ties_desc, uint64_t* id_lo, uint64_t* id_hi, d
   DevBuf<uint32_t> flag, pos; DevBuf<double> val;
   SB_TRY(flag.alloc(N + 1)); SB_TRY(pos.alloc(N + 1)); SB_TRY(val.alloc(N));
   SB_CUDA(cudaMemsetAsync(flag.p + N, 0, 4, s));
-  SB_LAUNCH(k_result_flags, div_up(N, 256), 256, 0, s, g->inv.p, g->kahan_sum.p, N, g->row_begin, g->row_end, (double)(N - 1), flag.p,
+  SB_LAUNCH(k_result_flags, div_up(N, 256), 256, 0, s, g->inv.p, g->kahan_sum.p, N, (uint64_t)0, N, (double)(N - 1), flag.p,
             val.p, 1u, 0u);
   SB_CHECK_LAUNCH();
   size_t need = 0;

@@ -464,13 +464,12 @@ def run_sharded_loop(engine, world_size, group=None, max_iters=0):
     entrypoint/ampc/harmonic_centrality/mapper.rs:38-45) for one rank, with torch.distributed as transport.
 
     `engine` owns this rank's shard: `step()` runs one HyperBall iteration over its destination rows,
-    `exchange_tensors()` exposes the full register array and changed bitmap as torch tensors,
-    `row_ranges()` gives every rank's row range.  After each step every owner broadcasts its rows (the DHT
-    `HyperLogLog64Upsert` max-merge has a single writer per row, so it is an all-gather) and its bitmap words
-    (SaveBloom/UpdateBloom), and the changed counts are summed (Meta.round_had_changes)."""
+    `exchange_tensors()` exposes the full register array and changed bitmap as torch tensors.  After each step
+    every owner broadcasts its rows (the DHT `HyperLogLog64Upsert` max-merge has a single writer per row, so it is
+    an all-gather) and its bitmap words (SaveBloom/UpdateBloom), and the changed counts are summed
+    (Meta.round_had_changes)."""
     import torch
     import torch.distributed as dist
-    ranges = engine.row_ranges()
     stats = []
     t = 0
     fused = bool(getattr(engine, "p2p", False))

@@ -1,6 +1,6 @@
 """Runs the path-1 GPU parity functions of tests/test_hyperball_gpu.py against the CPU SIMT emulation of the library
-(tests/emu/libsb200_emu.so).  Started as a subprocess by tests/test_hyperball_emulated.py so that switches read once
-per process (SB200_ARENA, SB200_STAGE_ROWPERM) can be varied.  argv[1]: "full" or "quick"."""
+(tests/emu/libsb200_emu.so).  Started as a subprocess by tests/test_hyperball_emulated.py so that a switch read once
+per process (SB200_ARENA) can be varied.  argv[1]: "full" or "quick"."""
 import ctypes as C
 import os
 import sys

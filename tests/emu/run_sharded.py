@@ -9,8 +9,6 @@ import ctypes as C
 import os
 import sys
 
-os.environ["SB200_SHARDED_PUSH"] = "1"   # the automatic switch to push on reused sharded handles is opt-in
-
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 sys.path.insert(0, os.path.dirname(HERE))

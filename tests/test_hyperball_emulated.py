@@ -2,8 +2,7 @@
 the emulator is and is not).  The parity functions are those of tests/test_hyperball_gpu.py: registers bit-exact after
 every iteration, KahanSum bit-exact, output ids and values bit-exact against the oracle, all three kernel families
 forced, rows that span several work items.  Besides checking the kernels under the largest lane skew a GPU may show,
-this runs both settings of the two staging switches (row-permutation CSR relabel vs second radix sort, slab arena vs the
-driver's stream-ordered pool)."""
+this runs both settings of the allocator switch (slab arena vs the driver's stream-ordered pool)."""
 import os
 import subprocess
 import sys
@@ -17,7 +16,7 @@ EMU = os.path.join(HERE, "emu")
 def _run(mode, **env):
     subprocess.check_call(["make", "-C", EMU], stdout=subprocess.DEVNULL)
     e = dict(os.environ)
-    for k in ("SB200_ARENA", "SB200_STAGE_ROWPERM", "SB200_ARENA_SLAB_MB"):
+    for k in ("SB200_ARENA", "SB200_ARENA_SLAB_MB"):
         e.pop(k, None)
     e.update(env)
     r = subprocess.run([sys.executable, os.path.join(EMU, "run_path1.py"), mode], env=e, capture_output=True, text=True, timeout=900)
@@ -27,11 +26,6 @@ def _run(mode, **env):
 
 def test_default_path_all_kernel_families():
     _run("full")
-
-
-def test_second_radix_sort_relabel():
-    """the row-permutation relabel is the default since round 2; SB200_STAGE_ROWPERM=0 is the second-sort path"""
-    _run("quick", SB200_STAGE_ROWPERM="0")
 
 
 def test_stream_ordered_pool_instead_of_arena():

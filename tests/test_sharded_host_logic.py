@@ -16,7 +16,7 @@ from stract_b200 import synth
 
 
 class NumpyShard:
-    """Owns destination rows [b, e) of a dense CSR; the full register array is replicated."""
+    """Owns the destination rows of its interleaved 32-row blocks; the full register array is replicated."""
 
     def __init__(self, d, rank, world):
         self.orc = DenseHyperBall(d["from_lo"], d["from_hi"], d["to_lo"], d["to_hi"], d["rel_flags"])
@@ -39,14 +39,10 @@ class NumpyShard:
             edges.append((a, b_))
         self.edges = np.array(edges, np.int64).reshape(-1, 2)
         # interleaved ownership: 32-row block b belongs to rank b % world (as in the CUDA library)
-        self.ranges = [0] * world + [n]
         self.own = ((np.arange(n) >> 5) % world) == rank
         self.regs = torch.from_numpy(self.orc.registers().reshape(-1).copy())
         self.front = torch.zeros((n + 31) // 32, dtype=torch.int32)
         self.changed_prev = np.ones(n, bool)
-
-    def row_ranges(self):
-        return self.ranges
 
     def step(self):
         old = self.regs.numpy().reshape(self.n, 64).copy()
