@@ -262,6 +262,82 @@ typedef struct { uint64_t candidates, matches, positions_decoded, position_bytes
 SB200_API int sb200_phrase_topk_batch(sb200_segment* seg, const sb200_phrase_batch* batch, uint32_t* docs, float* scores,
                                       uint32_t* n_out, sb200_phrase_stats* stats);
 
+/* ---- optic pattern rules as device docsets (core/src/query/pattern_query/, core/src/query/optic.rs) ----------------------
+ * A docset is a bitmap of ceil(max_doc / 32) u32 words in HBM (12.5 MB at 100 M docs), bit d = document d, on the device of
+ * the segment it was built from.  Optic rules only ever ask "is doc d in it?", so AND / OR of bitmaps is their exact
+ * composition (a rule = OR over its Matches blocks of the AND of the block's matchings, optic.rs:104-169). */
+typedef struct sb200_docset sb200_docset;
+#define SB200_PART_PAD 0u       /* padding behind a pattern's parts */
+#define SB200_PART_TERM 1u      /* PatternPart::Raw after tokenisation: one part per token, its ordinal in term_ords */
+#define SB200_PART_WILDCARD 2u  /* PatternPart::Wildcard */
+#define SB200_PART_ANCHOR 3u    /* PatternPart::Anchor */
+/* A batch of PatternQuerys over one field, parts as PatternQuery::new leaves them (every raw part tokenised into TERM parts).
+ * The library chooses PatternWeight::pattern_scorer's branch (weight.rs:121-226):
+ *   no parts -> empty;  no TERM and a WILDCARD -> every document;  no TERM, anchors only -> the documents whose token count is 0;
+ *   an SB200_ABSENT_TERM -> empty;  one TERM and nothing else -> its postings;
+ *   otherwise NormalPatternScorer (scorer.rs:203-339): the AND of the terms, then per document left = positions of term 0 and,
+ *   for every later TERM, left = { r in positions(term) : some l in left with r - slop <= l <= r } (saturating; slop 1, or
+ *   u32::MAX after a WILDCARD); the document matches when the last left is non-empty, an ANCHOR at index 0 holds (the first
+ *   position of term 0 is 0) and an ANCHOR at the last index holds (the last position of the last term equals
+ *   (token count - 1) as u32).  Anchors elsewhere are ignored.
+ * Row p has parts[p * n_parts ..] (SB200_PART_PAD behind) and the ordinals of its TERM parts in order in
+ * term_ords[p * n_terms ..]; at most SB200_MAX_QUERY_TERMS terms per pattern (SB200_ERANGE above).  Patterns with a TERM and
+ * another part need positions (sb200_segment_attach_positions); anchored and empty-field patterns need the token-count
+ * column (sb200_segment_attach_token_counts), else SB200_EINVAL.  out[p] receives a new docset per row. */
+typedef struct {
+  uint32_t n_patterns, n_parts;  /* n_parts = row width of parts */
+  const uint8_t* parts;          /* [n_patterns * n_parts] SB200_PART_* */
+  uint32_t n_terms, _pad;        /* row width of term_ords */
+  const uint32_t* term_ords;     /* [n_patterns * n_terms] ordinals or SB200_ABSENT_TERM; entries past the row's TERM count are ignored */
+} sb200_pattern_batch;
+/* candidates: documents holding every term of a positional pattern; matches: those that matched; positions_decoded /
+ * position_bytes as sb200_phrase_stats; ms: the whole call, kernel_ms: the launches (CUDA events). */
+typedef struct { uint64_t candidates, matches, positions_decoded, position_bytes; float ms, kernel_ms; } sb200_pattern_stats;
+SB200_API int sb200_pattern_docsets(sb200_segment* seg, const sb200_pattern_batch* batch, sb200_docset** out, sb200_pattern_stats* stats);
+/* The field's token-count fast field (NumTitleTokens, NumCleanBodyTokens, ...; weight.rs:129-160), one u64 per document, a
+ * missing value passed as 0 (EmptyFieldScorer's unwrap_or_default; NormalPatternScorer unwraps it, so an anchored pattern over
+ * a document without a value is outside the reference's domain).  Host or device memory; attaching again replaces it. */
+SB200_API int sb200_segment_attach_token_counts(sb200_segment* seg, const uint64_t* counts, uint32_t max_doc);
+/* the posting list of one term as a docset (FastSiteDomainPatternWeight: `|raw|` on Site / Domain reads the concatenated raw
+ * text in the no-tokenizer field, pattern_query/mod.rs:61-92,166-175; also any rule whose docset is one posting list).
+ * SB200_ABSENT_TERM gives the empty docset. */
+SB200_API int sb200_docset_from_postings(sb200_segment* seg, uint32_t term, sb200_docset** out);
+#define SB200_DOCSET_AND 0
+#define SB200_DOCSET_OR 1
+/* AND / OR of n >= 1 docsets with the same max_doc and device (fields of one tantivy segment) into a new docset */
+SB200_API int sb200_docset_combine(int op, const sb200_docset* const* inputs, uint32_t n, sb200_docset** out);
+SB200_API int sb200_docset_count(const sb200_docset* ds, uint64_t* count);
+/* the first min(cap, total) documents in ascending order into docs (host or device), the number of documents into *total */
+SB200_API int sb200_docset_read(const sb200_docset* ds, uint32_t* docs, uint64_t cap, uint64_t* total);
+SB200_API int sb200_docset_info(const sb200_docset* ds, uint32_t* max_doc, int* device);
+SB200_API void sb200_docset_destroy(sb200_docset* ds);
+
+/* The multi-field recall stage (sb200_multi_signal_topk_batch) with optic rules given as docsets.  Per query q:
+ *   rule_docset[q][r] (r < n_rules[q] <= SB200_MAX_OPTIC_RULES): an index into `docsets`, rule_boost[q][r] its f64 boost
+ *     (negative = downrank) -- SignalComputer's Boost / Downrank rules with b != 0 in rule order (computer/mod.rs:267-277).
+ *     A document in the rule's docset adds |b| to downrank or b to boost, in rule order; the total is multiplied by the
+ *     factor of sb200_multi_signal_topk_batch.
+ *   exclude[q]: a docset index or SB200_NO_DOCSET: the OR of the Discard rules and blocked hosts (MustNot).
+ *   require[q]: a docset index or SB200_NO_DOCSET: with DiscardNonMatching, the AND over optics of the OR of their non-Discard
+ *     rules (Must).
+ * A candidate in exclude or outside require is dropped before it is scored (query/mod.rs:129-137, optic.rs:50-89).  Rule
+ * slots (field | 0x80) and docset rules in one query are SB200_EINVAL: their relative order would be undefined.  Every docset
+ * must have the segment's max_doc and device.  An optic with no rules and no filters gives the bits of
+ * sb200_multi_signal_topk_batch. */
+#define SB200_MAX_OPTIC_RULES 64
+#define SB200_NO_DOCSET 0xFFFFFFFFu
+typedef struct {
+  uint32_t n_docsets, max_rules;        /* max_rules = row width of rule_docset / rule_boost */
+  const sb200_docset* const* docsets;   /* [n_docsets] */
+  const uint32_t* n_rules;              /* [n_queries]; NULL = no rules */
+  const uint32_t* rule_docset;          /* [n_queries * max_rules] */
+  const double* rule_boost;             /* [n_queries * max_rules] */
+  const uint32_t* exclude;              /* [n_queries]; NULL = none */
+  const uint32_t* require;              /* [n_queries]; NULL = none */
+} sb200_optic_batch;
+SB200_API int sb200_multi_signal_topk_batch_optic(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, uint32_t* docs,
+                                                  double* totals, uint32_t* n_out, sb200_bm25_stats* stats);
+
 /* idf(doc_freq, doc_count) = ln(1 + (N - n + 0.5) / (n + 0.5)) in f32 (tantivy/src/query/bm25.rs:52-56,
  * core/src/ranking/bm25.rs:23-27) for an array of doc_freqs; tantivy_weight != 0 returns Bm25Weight.weight = idf * (1 + K1). */
 SB200_API int sb200_bm25_idf(const uint32_t* doc_freq, uint64_t n, uint64_t doc_count, int tantivy_weight, float* out);

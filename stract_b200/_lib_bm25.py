@@ -56,6 +56,21 @@ class PhraseStats(C.Structure):
                 ("ms", C.c_float), ("kernel_ms", C.c_float)]
 
 
+class PatternBatch(C.Structure):
+    _fields_ = [("n_patterns", C.c_uint32), ("n_parts", C.c_uint32), ("parts", C.c_void_p), ("n_terms", C.c_uint32),
+                ("_pad", C.c_uint32), ("term_ords", C.c_void_p)]
+
+
+class PatternStats(C.Structure):
+    _fields_ = [("candidates", C.c_uint64), ("matches", C.c_uint64), ("positions_decoded", C.c_uint64), ("position_bytes", C.c_uint64),
+                ("ms", C.c_float), ("kernel_ms", C.c_float)]
+
+
+class OpticBatch(C.Structure):
+    _fields_ = [("n_docsets", C.c_uint32), ("max_rules", C.c_uint32), ("docsets", C.c_void_p), ("n_rules", C.c_void_p),
+                ("rule_docset", C.c_void_p), ("rule_boost", C.c_void_p), ("exclude", C.c_void_p), ("require", C.c_void_p)]
+
+
 def proto(L, f):
     vp, u32, u64, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int
     f("sb200_segment_create", i32, vp, u64, vp, u32, vp, u32, i32, i32, C.POINTER(vp))
@@ -80,3 +95,12 @@ def proto(L, f):
     f("sb200_positions_read", i32, vp, u32, u64, u32, vp)
     f("sb200_term_info_store_decode_positions", i32, vp, u64, i32, vp, vp, u64, C.POINTER(u64))
     f("sb200_phrase_topk_batch", i32, vp, C.POINTER(PhraseBatch), vp, vp, vp, C.POINTER(PhraseStats))
+    f("sb200_pattern_docsets", i32, vp, C.POINTER(PatternBatch), vp, C.POINTER(PatternStats))
+    f("sb200_segment_attach_token_counts", i32, vp, vp, u32)
+    f("sb200_docset_from_postings", i32, vp, u32, C.POINTER(vp))
+    f("sb200_docset_combine", i32, i32, vp, u32, C.POINTER(vp))
+    f("sb200_docset_count", i32, vp, C.POINTER(u64))
+    f("sb200_docset_read", i32, vp, vp, u64, C.POINTER(u64))
+    f("sb200_docset_info", i32, vp, C.POINTER(u32), C.POINTER(i32))
+    f("sb200_docset_destroy", None, vp)
+    f("sb200_multi_signal_topk_batch_optic", i32, C.POINTER(MultiSignalBatch), C.POINTER(OpticBatch), vp, vp, vp, C.POINTER(Bm25Stats))

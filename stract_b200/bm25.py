@@ -252,6 +252,12 @@ class SegmentReader:
         check(self._L.sb200_positions_read(self._h, int(term), int(offset), int(n), _p(out)))
         return out[:int(n)]
 
+    def attach_token_counts(self, counts):
+        """sb200_segment_attach_token_counts: the field's token-count fast field, one u64 per document (missing = 0)."""
+        c = np.ascontiguousarray(counts, np.uint64)
+        assert c.size == self.max_doc, "one token count per document"
+        check(self._L.sb200_segment_attach_token_counts(self._h, _p(c), self.max_doc))
+
     def info(self):
         si = B.SegmentInfo()
         check(self._L.sb200_segment_get_info(self._h, C.byref(si)))
@@ -267,6 +273,98 @@ class SegmentReader:
             self.close()
         except Exception:
             pass
+
+
+PART_PAD, PART_TERM, PART_WILDCARD, PART_ANCHOR = 0, 1, 2, 3
+MAX_QUERY_TERMS = 8
+MAX_OPTIC_RULES = 64
+NO_DOCSET = 0xFFFFFFFF
+
+
+class Docset:
+    """A device bitmap over one segment's documents (sb200_docset): what an optic rule's docset answers."""
+
+    def __init__(self, handle):
+        self._L = lib()
+        self._h = handle
+
+    @classmethod
+    def from_postings(cls, segment, term):
+        """The posting list of one term (FastSiteDomainPatternWeight); ABSENT_TERM gives the empty docset."""
+        h = C.c_void_p()
+        check(lib().sb200_docset_from_postings(segment._h, int(term), C.byref(h)))
+        return cls(h)
+
+    @classmethod
+    def combine(cls, op, docsets):
+        """AND ("and") / OR ("or") of docsets of one segment."""
+        arr = (C.c_void_p * len(docsets))(*[d._h.value for d in docsets])
+        h = C.c_void_p()
+        check(lib().sb200_docset_combine(0 if op == "and" else 1, C.cast(arr, C.c_void_p), len(docsets), C.byref(h)))
+        return cls(h)
+
+    def count(self):
+        n = C.c_uint64(0)
+        check(self._L.sb200_docset_count(self._h, C.byref(n)))
+        return int(n.value)
+
+    def docs(self, cap=None):
+        """The documents in ascending order (the first `cap` of them)."""
+        total = C.c_uint64(0)
+        check(self._L.sb200_docset_read(self._h, None, 0, C.byref(total)))
+        n = int(total.value) if cap is None else min(int(cap), int(total.value))
+        out = np.zeros(max(n, 1), np.uint32)
+        check(self._L.sb200_docset_read(self._h, _p(out), n, C.byref(total)))
+        return out[:n]
+
+    def close(self):
+        if self._h:
+            self._L.sb200_docset_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def pattern_docsets(segment, patterns, return_stats=False):
+    """sb200_pattern_docsets: `patterns` = [(parts, term_ords)] with parts a sequence of PART_TERM / PART_WILDCARD / PART_ANCHOR
+    and term_ords the ordinals of the TERM parts (ABSENT_TERM for a token the segment lacks).  One Docset per pattern."""
+    n = len(patterns)
+    for parts, ords in patterns:
+        if sum(1 for x in parts if x == PART_TERM) > MAX_QUERY_TERMS:
+            raise ValueError(f"a pattern has more than {MAX_QUERY_TERMS} terms")
+    npw = max([len(p) for p, _ in patterns] + [1]); ntw = max([len(o) for _, o in patterns] + [1])
+    parts = np.zeros((max(n, 1), npw), np.uint8); ords = np.full((max(n, 1), ntw), NO_TERM, np.uint32)
+    for i, (p, o) in enumerate(patterns):
+        parts[i, :len(p)] = p
+        ords[i, :len(o)] = o
+    pb = B.PatternBatch()
+    pb.n_patterns, pb.n_parts, pb.parts, pb.n_terms, pb.term_ords = n, npw, _p(parts), ntw, _p(ords)
+    hs = (C.c_void_p * max(n, 1))()
+    st = B.PatternStats()
+    check(segment._L.sb200_pattern_docsets(segment._h, C.byref(pb), C.cast(hs, C.c_void_p), C.byref(st)))
+    out = [Docset(C.c_void_p(hs[i])) for i in range(n)]
+    if return_stats:
+        return out, {k: getattr(st, k) for k, _ in B.PatternStats._fields_}
+    return out
+
+
+class OpticTables:
+    """The per-query optic inputs of the recall stage (sb200_optic_batch): `docsets` (Docset list), per query the rule docset
+    indices with their f64 boosts in rule order, and the exclude / require docset indices (None = no filter)."""
+
+    def __init__(self, docsets, rules, exclude=None, require=None):
+        self.docsets = list(docsets)
+        self.rules = [list(r) for r in rules]           # per query [(docset index, boost)]
+        nq = len(self.rules)
+        self.exclude = [None] * nq if exclude is None else list(exclude)
+        self.require = [None] * nq if require is None else list(require)
+        for r in self.rules:
+            if len(r) > MAX_OPTIC_RULES:
+                raise ValueError(f"a query has {len(r)} optic rules; at most {MAX_OPTIC_RULES}")
 
 
 class SignalTable:
@@ -742,12 +840,14 @@ class MultiFieldSignalComputer:
                 c = self.coefficient(name, coef)
         return c
 
-    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None):
+    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None, optic=None):
         """slot_field / slot_term [n_queries, n_slots]: field index into `self.names` (TextFieldEnum order; 0xFF pads) and the term's ordinal in that
         field's reader (NO_TERM = the segment does not hold it).  idf comes from the field's own doc_freq
         (MultiBm25Weight::for_terms), the Bm25F idf from `doc_freq_all_body` [n_queries, n_slots] (WeightCache: the AllBody
         doc_freq of the token), defaulting to the field's own.  Optic rules: a slot with field | 0x80 is the docset of a rule,
-        `slot_boost` [n_queries, n_slots] holds its boost (negative = downrank): SignalComputer::boosts (mod.rs:471-497)."""
+        `slot_boost` [n_queries, n_slots] holds its boost (negative = downrank): SignalComputer::boosts (mod.rs:471-497).
+        `optic` (OpticTables, e.g. from stract_b200.optic.compile_optics): optic rules as device docsets, with the Discard /
+        DiscardNonMatching filters (sb200_multi_signal_topk_batch_optic); None keeps sb200_multi_signal_topk_batch."""
         sf = np.ascontiguousarray(slot_field, np.uint8); st = np.ascontiguousarray(slot_term, np.uint32)
         nq, ns = sf.shape
         idf1 = np.zeros((nq, ns), np.float32); idf2 = np.zeros((nq, ns), np.float32)
@@ -782,7 +882,24 @@ class MultiFieldSignalComputer:
         sbst = None if slot_boost is None else np.ascontiguousarray(slot_boost, np.float64)
         mb.slot_boost = _p(sbst)
         stt = B.Bm25Stats()
-        check(self._L.sb200_multi_signal_topk_batch(C.byref(mb), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+        if optic is None:
+            check(self._L.sb200_multi_signal_topk_batch(C.byref(mb), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+        else:
+            if len(optic.rules) != nq:
+                raise ValueError(f"optic tables for {len(optic.rules)} queries, batch has {nq}")
+            mr = max([len(r) for r in optic.rules] + [1])
+            nr = np.array([len(r) for r in optic.rules], np.uint32)
+            rd = np.zeros((nq, mr), np.uint32); rb = np.zeros((nq, mr), np.float64)
+            for q, r in enumerate(optic.rules):
+                for j, (d, b) in enumerate(r):
+                    rd[q, j] = d; rb[q, j] = b
+            nd = lambda v: NO_DOCSET if v is None else int(v)
+            ex = np.array([nd(v) for v in optic.exclude], np.uint32); rq = np.array([nd(v) for v in optic.require], np.uint32)
+            darr = (C.c_void_p * max(len(optic.docsets), 1))(*[d._h.value for d in optic.docsets])
+            ob = B.OpticBatch()
+            ob.n_docsets, ob.max_rules, ob.docsets = len(optic.docsets), mr, C.cast(darr, C.c_void_p)
+            ob.n_rules, ob.rule_docset, ob.rule_boost, ob.exclude, ob.require = _p(nr), _p(rd), _p(rb), _p(ex), _p(rq)
+            check(self._L.sb200_multi_signal_topk_batch_optic(C.byref(mb), C.byref(ob), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
         self.last_inputs = dict(idf=idf1, idf_f=idf2, caches=caches)
         if return_stats:
             return docs, totals, n_out, {k_: getattr(stt, k_) for k_, _ in B.Bm25Stats._fields_ if not k_.startswith("_")}

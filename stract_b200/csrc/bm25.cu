@@ -20,6 +20,8 @@
 //   Block-WAND replay    k_wand (bm25_wand.cuh), one warp per query in the reference's pruning and summation order.
 //   multi-field signals  k_sig_multi<TMAX> (bm25_multi.cuh).
 //   phrases              k_phrase_cand + k_phrase_verify + k_and3_select (bm25_phrase.cuh).
+//   optic pattern docsets k_phrase_cand + k_pattern_verify and word kernels (bm25_pattern.cuh); k_sig_multi<TMAX, true>
+//                        consumes them in the recall stage.
 // A query of the walk kernels much larger than the batch average is cut into doc-range work items (plan_items);
 // k_merge_topk merges their partial top-k lists.  Keys are (order-preserving score bits, ~doc), so the result order
 // is the reference's (score desc, doc asc) total order.
@@ -95,6 +97,18 @@ struct sb200_segment {
   sb200::DevBuf<float> ph_weight;
   sb200::DevBuf<uint64_t> ph_coff, ph_pre;
   sb200::DevBuf<unsigned long long> ph_ov, ph_ovc;
+  // token-count fast field of the field (sb200_segment_attach_token_counts, bm25_pattern.cuh)
+  bool has_tok = false;
+  sb200::DevBuf<uint64_t> tok_count;
+  // scratch of the pattern path and of the optic recall stage (the latter in the first field's handle)
+  sb200::DevBuf<uint32_t> pt_col, pt_nparts; sb200::DevBuf<uint8_t> pt_parts; sb200::DevBuf<uint64_t> pt_bits;
+  sb200::DevBuf<uint64_t> o_bits; sb200::DevBuf<uint32_t> o_nrules, o_rule, o_exclude, o_require; sb200::DevBuf<double> o_boost;
+};
+
+struct sb200_docset {
+  int device = 0;
+  uint32_t max_doc = 0;
+  sb200::DevBuf<uint32_t> bits;   // ceil(max_doc / 32) words
 };
 
 namespace sb200 {
@@ -253,6 +267,7 @@ static int launch_topk_warp(const WParams& P, cudaStream_t s) {
 #include "bm25_multi.cuh"
 #include "bm25_wand.cuh"
 #include "bm25_phrase.cuh"
+#include "bm25_pattern.cuh"
 namespace sb200 {
 
 static void seg_view(const sb200_segment* g, SegView& S) {
@@ -291,17 +306,18 @@ static void plan_items(const std::vector<uint64_t>& work, const std::vector<uint
   if (!pl.jobs.empty()) { pl.capm = 1024; while (pl.capm < wmax * k) pl.capm <<= 1; }
 }
 
-template <int TMAX>
+template <int TMAX, bool OPTIC>
 static int launch_multi(const MParams& P, cudaStream_t s) {
   const size_t sm = m_cta_smem<TMAX>();
   static bool configured = false;
-  if (!configured) { SB_CUDA(cudaFuncSetAttribute(k_sig_multi<TMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); configured = true; }
-  SB_LAUNCH(k_sig_multi<TMAX>, div_up(P.n_items, WQ), WQ * 32, sm, s, P);
+  if (!configured) { SB_CUDA(cudaFuncSetAttribute(k_sig_multi<TMAX, OPTIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); configured = true; }
+  SB_LAUNCH((k_sig_multi<TMAX, OPTIC>), div_up(P.n_items, WQ), WQ * 32, sm, s, P);
   SB_CHECK_LAUNCH();
   return SB200_OK;
 }
 
-static int run_multi(const sb200_multi_signal_batch* b, uint32_t* docs, double* totals, uint32_t* n_out, sb200_bm25_stats* stats) {
+static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch* ob, uint32_t* docs, double* totals, uint32_t* n_out,
+                     sb200_bm25_stats* stats) {
   if (!b || !b->fields || !b->ops || !b->slot_field || !b->slot_term || !b->slot_idf || !b->slot_idf_f || !docs || !totals || !n_out)
     SB_FAIL(SB200_EINVAL, "NULL argument");
   const uint32_t nq = b->n_queries, SM = b->n_slots, k = b->k, NF = b->n_fields, NO = b->n_ops;
@@ -329,6 +345,26 @@ static int run_multi(const sb200_multi_signal_batch* b, uint32_t* docs, double* 
     }
   }
   if (n_cols && b->signals->max_doc < g->max_doc) SB_FAIL(SB200_EINVAL, "signal table covers %u docs, segment has %u", b->signals->max_doc, g->max_doc);
+  if (ob) {   // optic docsets: shapes, indices, devices; rule slots and docset rules never share a query
+    if (ob->n_docsets && !ob->docsets) SB_FAIL(SB200_EINVAL, "optic: NULL docsets");
+    if (ob->n_rules && (!ob->rule_docset || !ob->rule_boost)) SB_FAIL(SB200_EINVAL, "optic: NULL rule_docset / rule_boost");
+    if (ob->n_rules && (ob->max_rules == 0 || ob->max_rules > SB200_MAX_OPTIC_RULES)) SB_FAIL(SB200_ERANGE, "optic: max_rules %u outside [1,%d]", ob->max_rules, SB200_MAX_OPTIC_RULES);
+    for (uint32_t i = 0; i < ob->n_docsets; i++) {
+      const sb200_docset* d = ob->docsets[i];
+      if (!d) SB_FAIL(SB200_EINVAL, "optic: docset %u is NULL", i);
+      if (d->max_doc != g->max_doc || d->device != g->device) SB_FAIL(SB200_EINVAL, "optic: docset %u has max_doc %u on device %d, the segment %u on %d", i, d->max_doc, d->device, g->max_doc, g->device);
+    }
+    for (uint32_t q = 0; q < nq; q++) {
+      const uint32_t nr = ob->n_rules ? ob->n_rules[q] : 0u;
+      if (nr > ob->max_rules || nr > SB200_MAX_OPTIC_RULES) SB_FAIL(SB200_ERANGE, "optic: query %u has %u rules (max %u)", q, nr, std::min<uint32_t>(ob->max_rules, SB200_MAX_OPTIC_RULES));
+      for (uint32_t r = 0; r < nr; r++) if (ob->rule_docset[(size_t)q * ob->max_rules + r] >= ob->n_docsets) SB_FAIL(SB200_EINVAL, "optic: query %u rule %u: docset index out of range", q, r);
+      for (const uint32_t* f : {ob->exclude, ob->require}) if (f && f[q] != SB200_NO_DOCSET && f[q] >= ob->n_docsets) SB_FAIL(SB200_EINVAL, "optic: query %u: filter docset index out of range", q);
+      if (nr) for (uint32_t x = 0; x < SM; x++) {
+        const uint8_t f = b->slot_field[(size_t)q * SM + x];
+        if (f != 0xFF && (f & 0x80)) SB_FAIL(SB200_EINVAL, "optic: query %u mixes rule slots and docset rules (their order would be undefined)", q);
+      }
+    }
+  }
   if (nq == 0) return SB200_OK;
   // planning: slots keep their query order (the f32 sums depend on it); padding slots (field 0xFF) are dropped
   std::vector<uint8_t> sf((size_t)nq * SM, 0);
@@ -412,8 +448,32 @@ static int run_multi(const sb200_multi_signal_batch* b, uint32_t* docs, double* 
   P.n_items = n_items; P.item_q = g->q_items.p; P.item_lo = g->q_items.p + n_items; P.item_hi = g->q_items.p + 2 * (size_t)n_items; P.item_out = g->q_items.p + 3 * (size_t)n_items;
   if (n_cols) { P.sig = b->signals->rows.p; P.n_cols = n_cols; }
   P.g_khi = g->g_khi.p; P.g_klo = g->g_klo.p; P.o_docs = g->o_docs.p; P.o_totals = g->o_totals.p; P.o_n = g->o_n.p; P.counters = g->counters.p;
+  std::vector<uint64_t> bp; std::vector<uint32_t> nr, ex, rq, rd; std::vector<double> rb;   // optic tables, alive until the sync
+  if (ob) {
+    bp.assign(std::max<uint32_t>(ob->n_docsets, 1), 0);
+    for (uint32_t i = 0; i < ob->n_docsets; i++) bp[i] = (uint64_t)(uintptr_t)ob->docsets[i]->bits.p;
+    const uint32_t MR = ob->n_rules ? ob->max_rules : 1u;
+    nr.assign(nq, 0); ex.assign(nq, SB200_NO_DOCSET); rq.assign(nq, SB200_NO_DOCSET); rd.assign((size_t)nq * MR, 0); rb.assign((size_t)nq * MR, 0.0);
+    for (uint32_t q = 0; q < nq; q++) {
+      nr[q] = ob->n_rules ? ob->n_rules[q] : 0u;
+      if (ob->exclude) ex[q] = ob->exclude[q];
+      if (ob->require) rq[q] = ob->require[q];
+      for (uint32_t r = 0; r < nr[q]; r++) { rd[(size_t)q * MR + r] = ob->rule_docset[(size_t)q * MR + r]; rb[(size_t)q * MR + r] = ob->rule_boost[(size_t)q * MR + r]; }
+    }
+    SB_TRY(ensure(g->o_bits, bp.size())); SB_TRY(ensure(g->o_nrules, nq)); SB_TRY(ensure(g->o_exclude, nq)); SB_TRY(ensure(g->o_require, nq));
+    SB_TRY(ensure(g->o_rule, rd.size())); SB_TRY(ensure(g->o_boost, rb.size()));
+    SB_CUDA(cudaMemcpyAsync(g->o_bits.p, bp.data(), bp.size() * 8, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->o_nrules.p, nr.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->o_exclude.p, ex.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->o_require.p, rq.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->o_rule.p, rd.data(), rd.size() * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->o_boost.p, rb.data(), rb.size() * 8, cudaMemcpyHostToDevice, s));
+    P.d_bits = (const uint32_t* const*)g->o_bits.p; P.d_nrules = g->o_nrules.p; P.d_rule = g->o_rule.p; P.d_boost = g->o_boost.p;
+    P.d_max_rules = MR; P.d_exclude = g->o_exclude.p; P.d_require = g->o_require.p;
+  }
   SB_CUDA(cudaEventRecord(g->evk0, s));
-  if (SM <= 8) SB_TRY(launch_multi<8>(P, s)); else SB_TRY(launch_multi<16>(P, s));
+  if (ob) { if (SM <= 8) SB_TRY((launch_multi<8, true>(P, s))); else SB_TRY((launch_multi<16, true>(P, s))); }
+  else if (SM <= 8) SB_TRY((launch_multi<8, false>(P, s))); else SB_TRY((launch_multi<16, false>(P, s)));
   if (!pl.jobs.empty()) {
     const size_t msm = (size_t)pl.capm * 12;
     static size_t mconf = 0;
@@ -786,7 +846,7 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
   if (sel_conf < sel_smem) { SB_CUDA(cudaFuncSetAttribute(k_and3_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem)); sel_conf = sel_smem; }
   const size_t cand_smem = (size_t)A3_WARPS * nt * 128 * 12;
   static size_t cand_conf = 0;
-  if (cand_conf < cand_smem) { SB_CUDA(cudaFuncSetAttribute(k_phrase_cand, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand_smem)); cand_conf = cand_smem; }
+  if (cand_conf < cand_smem) { SB_CUDA(cudaFuncSetAttribute(k_phrase_cand<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand_smem)); cand_conf = cand_smem; }
   int n_sm = 132;
   { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 132; }
   // candidate records: doc + nt x (u64 offset, u32 tf) + a match (key, doc) per entry
@@ -832,7 +892,7 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
       C.A.units = (const AUnit*)g->a3_units.p; C.A.n_units = n_units;
       C.A.cand_off = g->a3_off.p; C.A.cand_cnt = g->a3_cnt.p; C.A.counters = g->counters.p;
       C.pos_base = g->pos_base.p; C.nt = nt; C.c_doc = g->ph_cdoc.p; C.c_off = g->ph_coff.p; C.c_tf = g->ph_ctf.p;
-      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_cand, div_up(n_units, A3_WARPS), A3_WARPS * 32, cand_smem, s, C); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_cand<2>, div_up(n_units, A3_WARPS), A3_WARPS * 32, cand_smem, s, C); SB_CHECK_LAUNCH(); return SB200_OK; }));
     }
     // candidate counts -> the group's prefix (k_phrase_verify maps a candidate to its query by a binary search in it)
     SB_CUDA(cudaMemcpyAsync(cnt.data() + g0, g->a3_cnt.p + g0, (size_t)(g1 - g0) * 4, cudaMemcpyDeviceToHost, s));
@@ -893,6 +953,240 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
     stats->candidates = h[0]; stats->matches = h[1]; stats->positions_decoded = h[3]; stats->position_bytes = h[4];
     cudaEventElapsedTime(&stats->ms, g->ev0, g->ev1); stats->kernel_ms = kms;
   }
+  return SB200_OK;
+}
+
+
+// A new, zeroed docset over the segment's documents
+static int docset_new(const sb200_segment* g, sb200_docset** out) {
+  sb200_docset* d = new (std::nothrow) sb200_docset;
+  if (!d) SB_FAIL(SB200_ENOMEM, "docset: host allocation failed");
+  d->device = g->device; d->max_doc = g->max_doc;
+  const size_t nw = std::max<size_t>(((size_t)g->max_doc + 31) / 32, 1);
+  int rc = d->bits.alloc(nw);
+  if (rc == SB200_OK && cudaMemsetAsync(d->bits.p, 0, nw * 4, g->stream) != cudaSuccess) { set_error("docset: memset failed"); rc = SB200_ECUDA; }
+  if (rc != SB200_OK) { delete d; return rc; }
+  *out = d;
+  return SB200_OK;
+}
+
+// Pattern batch (bm25_pattern.cuh).  Host planning is PatternWeight::pattern_scorer's branch choice; positional patterns go
+// through k_phrase_cand (terms in Intersection order: stable sort by doc_freq) and k_pattern_verify in groups whose candidate
+// records fit a memory budget, like run_phrase.
+static int run_patterns(sb200_segment* g, const sb200_pattern_batch* b, sb200_docset** out, sb200_pattern_stats* stats) {
+  NvtxRange nvtx("sb200 pattern docsets");
+  cudaStream_t s = g->stream;
+  if (!b || !out || (b->n_patterns && b->n_parts && !b->parts)) SB_FAIL(SB200_EINVAL, "NULL argument");
+  const uint32_t np_ = b->n_patterns, NP = b->n_parts, NT = b->n_terms;
+  if (NT > (uint32_t)MAXT) SB_FAIL(SB200_ERANGE, "n_terms %u above %d", NT, MAXT);
+  if (NT && !b->term_ords) SB_FAIL(SB200_EINVAL, "NULL term_ords");
+  if (stats) memset(stats, 0, sizeof(*stats));
+  enum { EMPTY, ALL, EMPTY_FIELD, POSTINGS, NORMAL };
+  std::vector<int> kind(np_, EMPTY);
+  std::vector<uint32_t> nparts(np_, 0), nterms(np_, 0);
+  for (uint32_t p = 0; p < np_; p++) {
+    uint32_t n = 0, t = 0; bool wild = false, anchor = false, absent = false;
+    for (uint32_t i = 0; i < NP; i++) {
+      const uint8_t x = b->parts[(size_t)p * NP + i];
+      if (x == SB200_PART_PAD) {
+        for (uint32_t j = i; j < NP; j++) if (b->parts[(size_t)p * NP + j] != SB200_PART_PAD) SB_FAIL(SB200_EINVAL, "pattern %u: SB200_PART_PAD pads the end of a row only", p);
+        break;
+      }
+      if (x > SB200_PART_ANCHOR) SB_FAIL(SB200_EINVAL, "pattern %u part %u: kind %u", p, i, (unsigned)x);
+      if (x == SB200_PART_TERM) {
+        if (t >= (uint32_t)MAXT) SB_FAIL(SB200_ERANGE, "pattern %u has more than %d terms", p, MAXT);
+        if (t >= NT) SB_FAIL(SB200_EINVAL, "pattern %u has more TERM parts than the row width n_terms %u", p, NT);
+        const uint32_t ord = b->term_ords[(size_t)p * NT + t];
+        if (ord == SB200_ABSENT_TERM) absent = true;
+        else if (ord >= g->n_terms) SB_FAIL(SB200_EINVAL, "pattern %u: term ordinal %u >= %u", p, ord, g->n_terms);
+        t++;
+      }
+      wild |= x == SB200_PART_WILDCARD; anchor |= x == SB200_PART_ANCHOR;
+      n++;
+    }
+    nparts[p] = n; nterms[p] = t;
+    if (n == 0) kind[p] = EMPTY;
+    else if (t == 0 && wild) kind[p] = ALL;
+    else if (t == 0) kind[p] = EMPTY_FIELD;
+    else if (absent) kind[p] = EMPTY;
+    else if (t == 1 && n == 1) kind[p] = POSTINGS;
+    else kind[p] = NORMAL;
+    if ((kind[p] == EMPTY_FIELD || (kind[p] == NORMAL && anchor)) && !g->has_tok)
+      SB_FAIL(SB200_EINVAL, "pattern %u needs the field's token counts (sb200_segment_attach_token_counts)", p);
+    if (kind[p] == NORMAL && (g->record != SB200_RECORD_FREQS_POSITIONS || !g->has_pos))
+      SB_FAIL(SB200_EINVAL, "pattern %u needs positions (record option 2 and sb200_segment_attach_positions)", p);
+  }
+  for (uint32_t p = 0; p < np_; p++) out[p] = nullptr;
+  // every docset is created first; on an error the ones made so far are destroyed
+  auto fail_cleanup = [&](int rc) { for (uint32_t p = 0; p < np_; p++) { delete out[p]; out[p] = nullptr; } return rc; };
+  for (uint32_t p = 0; p < np_; p++) { const int rc = docset_new(g, &out[p]); if (rc != SB200_OK) return fail_cleanup(rc); }
+  if (np_ == 0) return SB200_OK;
+  int rc = [&]() -> int {
+    const uint32_t nw = (g->max_doc + 31) / 32;
+    float kms = 0.0f;
+    auto timed = [&](auto&& launch) -> int {
+      SB_CUDA(cudaEventRecord(g->evk0, s));
+      SB_TRY(launch());
+      SB_CUDA(cudaEventRecord(g->evk1, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+      return SB200_OK;
+    };
+    SB_CUDA(cudaEventRecord(g->ev0, s));
+    SB_TRY(ensure(g->counters, 8));
+    SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 8 * sizeof(unsigned long long), s));
+    // word kernels
+    for (uint32_t p = 0; p < np_; p++) {
+      if (kind[p] == ALL) SB_TRY(timed([&]() -> int { SB_LAUNCH(k_docset_all, div_up(nw, 256), 256, 0, s, out[p]->bits.p, g->max_doc); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      if (kind[p] == EMPTY_FIELD) SB_TRY(timed([&]() -> int { SB_LAUNCH(k_docset_empty_field, div_up(nw, 256), 256, 0, s, g->tok_count.p, out[p]->bits.p, g->max_doc); SB_CHECK_LAUNCH(); return SB200_OK; }));
+    }
+    // one-term shortcuts: every posting, one launch for all of them
+    std::vector<uint32_t> pq;   // query slot -> pattern
+    for (uint32_t p = 0; p < np_; p++) if (kind[p] == POSTINGS) pq.push_back(p);
+    SB_TRY(ensure(g->pt_bits, std::max<size_t>(np_, 1)));
+    SB_TRY(ensure(g->q_weights, std::max<size_t>((size_t)np_ * std::max<uint32_t>(NT, 1), 1)));
+    SB_CUDA(cudaMemsetAsync(g->q_weights.p, 0, std::max<size_t>((size_t)np_ * std::max<uint32_t>(NT, 1), 1) * 4, s));
+    std::vector<uint64_t> bp(np_);
+    if (!pq.empty()) {
+      const uint32_t n1 = (uint32_t)pq.size();
+      std::vector<uint32_t> terms(n1), ones(n1, 1);
+      std::vector<AUnit> units;
+      for (uint32_t i = 0; i < n1; i++) {
+        const uint32_t p = pq[i];
+        terms[i] = b->term_ords[(size_t)p * NT];
+        bp[i] = (uint64_t)(uintptr_t)out[p]->bits.p;
+        const uint32_t df = g->h_df[terms[i]], nblk = (df >> 7) + ((df & 127u) ? 1u : 0u);
+        for (uint32_t b0 = 0; b0 < nblk; b0 += A3_UNIT_BLOCKS) { AUnit u; u.q = i; u.blk_lo = b0; u.blk_hi = std::min(nblk, b0 + A3_UNIT_BLOCKS); u._pad = 0; units.push_back(u); }
+      }
+      SB_TRY(ensure(g->q_terms, n1)); SB_TRY(ensure(g->q_nterms, n1)); SB_TRY(ensure(g->a3_units, std::max<size_t>(units.size(), 1)));
+      SB_CUDA(cudaMemcpyAsync(g->q_terms.p, terms.data(), (size_t)n1 * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, ones.data(), (size_t)n1 * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->pt_bits.p, bp.data(), (size_t)n1 * 8, cudaMemcpyHostToDevice, s));
+      if (!units.empty()) {
+        SB_CUDA(cudaMemcpyAsync(g->a3_units.p, units.data(), units.size() * sizeof(AUnit), cudaMemcpyHostToDevice, s));
+        A3Params A;
+        memset(&A, 0, sizeof(A));
+        seg_view(g, A.S); A.a128 = g->a_post.p; A.t_aoff = g->t_aoff.p;
+        A.q_terms = g->q_terms.p; A.q_nterms = g->q_nterms.p; A.q_weights = g->q_weights.p; A.n_terms_max = 1;
+        A.units = (const AUnit*)g->a3_units.p; A.n_units = (uint32_t)units.size(); A.counters = g->counters.p;
+        SB_TRY(timed([&]() -> int { SB_LAUNCH(k_docset_postings, div_up(A.n_units, A3_WARPS), A3_WARPS * 32, 0, s, A, (uint32_t* const*)g->pt_bits.p); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      }
+      SB_CUDA(cudaStreamSynchronize(s));   // the host tables above are reused by the positional patterns
+    }
+    // positional patterns
+    std::vector<uint32_t> nq_p;
+    for (uint32_t p = 0; p < np_; p++) if (kind[p] == NORMAL) nq_p.push_back(p);
+    const uint32_t nq = (uint32_t)nq_p.size(), nt = std::max<uint32_t>(NT, 1), npw = std::max<uint32_t>(NP, 1);
+    if (nq) {
+      std::vector<uint32_t> terms((size_t)nq * nt, 0), col((size_t)nq * nt, 0), nt_q(nq, 0), np_q(nq, 0);
+      std::vector<uint8_t> parts((size_t)nq * npw, 0);
+      for (uint32_t i = 0; i < nq; i++) {
+        const uint32_t p = nq_p[i], c = nterms[p];
+        uint32_t idx[MAXT];
+        for (uint32_t j = 0; j < c; j++) idx[j] = j;
+        const uint32_t* ords = b->term_ords + (size_t)p * NT;
+        std::stable_sort(idx, idx + c, [&](uint32_t x, uint32_t y) { return g->h_df[ords[x]] < g->h_df[ords[y]]; });
+        for (uint32_t r = 0; r < c; r++) { terms[(size_t)i * nt + r] = ords[idx[r]]; col[(size_t)i * nt + idx[r]] = r; }
+        for (uint32_t j = 0; j < nparts[p]; j++) parts[(size_t)i * npw + j] = b->parts[(size_t)p * NP + j];
+        nt_q[i] = c; np_q[i] = nparts[p];
+        bp[i] = (uint64_t)(uintptr_t)out[p]->bits.p;
+      }
+      SB_TRY(ensure(g->q_terms, terms.size())); SB_TRY(ensure(g->pt_col, col.size())); SB_TRY(ensure(g->q_nterms, nq));
+      SB_TRY(ensure(g->pt_nparts, nq)); SB_TRY(ensure(g->pt_parts, parts.size()));
+      SB_TRY(ensure(g->a3_off, nq)); SB_TRY(ensure(g->a3_cnt, nq)); SB_TRY(ensure(g->ph_ovc, 4)); SB_TRY(ensure(g->ph_pre, (size_t)nq + 1));
+      SB_CUDA(cudaMemcpyAsync(g->q_terms.p, terms.data(), terms.size() * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->pt_col.p, col.data(), col.size() * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, nt_q.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->pt_nparts.p, np_q.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->pt_parts.p, parts.data(), parts.size(), cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemcpyAsync(g->pt_bits.p, bp.data(), (size_t)nq * 8, cudaMemcpyHostToDevice, s));
+      SB_CUDA(cudaMemsetAsync(g->a3_cnt.p, 0, (size_t)nq * 4, s));
+      const size_t cand_smem = (size_t)A3_WARPS * nt * 128 * 12;
+      static size_t cand_conf = 0;
+      if (cand_conf < cand_smem) { SB_CUDA(cudaFuncSetAttribute(k_phrase_cand<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand_smem)); cand_conf = cand_smem; }
+      int n_sm = 132;
+      { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 132; }
+      uint64_t budget = (uint64_t)2 << 30;   // candidate records: doc + nt x (u64 offset, u32 tf)
+      const uint64_t max_entries = std::max<uint64_t>(budget / (4 + 12 * (uint64_t)nt), 1);
+      std::vector<uint64_t> off(nq, 0), pre(nq + 1, 0);
+      std::vector<uint32_t> cnt(nq, 0);
+      std::vector<AUnit> units;
+      uint32_t g0 = 0;
+      while (g0 < nq) {
+        uint64_t entries = 0; uint32_t g1 = g0;
+        units.clear();
+        while (g1 < nq) {
+          const uint32_t dfA = g->h_df[terms[(size_t)g1 * nt]];
+          if (g1 > g0 && entries + dfA > max_entries) break;
+          off[g1] = entries; entries += dfA;
+          const uint32_t nblk = (dfA >> 7) + ((dfA & 127u) ? 1u : 0u);
+          for (uint32_t b0 = 0; b0 < nblk; b0 += A3_UNIT_BLOCKS) { AUnit u; u.q = g1; u.blk_lo = b0; u.blk_hi = std::min(nblk, b0 + A3_UNIT_BLOCKS); u._pad = 0; units.push_back(u); }
+          g1++;
+        }
+        const uint32_t n_units = (uint32_t)units.size();
+        const size_t ne = (size_t)std::max<uint64_t>(entries, 1);
+        SB_TRY(ensure(g->ph_cdoc, ne)); SB_TRY(ensure(g->ph_coff, ne * nt)); SB_TRY(ensure(g->ph_ctf, ne * nt));
+        SB_TRY(ensure(g->a3_units, std::max<size_t>(n_units, 1)));
+        SB_CUDA(cudaMemcpyAsync(g->a3_off.p + g0, off.data() + g0, (size_t)(g1 - g0) * 8, cudaMemcpyHostToDevice, s));
+        if (n_units) {
+          SB_CUDA(cudaMemcpyAsync(g->a3_units.p, units.data(), (size_t)n_units * sizeof(AUnit), cudaMemcpyHostToDevice, s));
+          PhCandParams C;
+          memset(&C, 0, sizeof(C));
+          seg_view(g, C.A.S); C.A.a128 = g->a_post.p; C.A.t_aoff = g->t_aoff.p;
+          C.A.q_terms = g->q_terms.p; C.A.q_nterms = g->q_nterms.p; C.A.q_weights = g->q_weights.p; C.A.n_terms_max = nt;
+          C.A.units = (const AUnit*)g->a3_units.p; C.A.n_units = n_units;
+          C.A.cand_off = g->a3_off.p; C.A.cand_cnt = g->a3_cnt.p; C.A.counters = g->counters.p;
+          C.pos_base = g->pos_base.p; C.nt = nt; C.c_doc = g->ph_cdoc.p; C.c_off = g->ph_coff.p; C.c_tf = g->ph_ctf.p;
+          SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_cand<1>, div_up(n_units, A3_WARPS), A3_WARPS * 32, cand_smem, s, C); SB_CHECK_LAUNCH(); return SB200_OK; }));
+        }
+        SB_CUDA(cudaMemcpyAsync(cnt.data() + g0, g->a3_cnt.p + g0, (size_t)(g1 - g0) * 4, cudaMemcpyDeviceToHost, s));
+        SB_CUDA(cudaStreamSynchronize(s));
+        const uint32_t ns = g1 - g0;
+        pre[0] = 0;
+        for (uint32_t i = 0; i < ns; i++) pre[i + 1] = pre[i] + cnt[g0 + i];
+        const uint64_t total = pre[ns];
+        if (total) {
+          SB_CUDA(cudaMemcpyAsync(g->ph_pre.p, pre.data(), (size_t)(ns + 1) * 8, cudaMemcpyHostToDevice, s));
+          SB_TRY(ensure(g->ph_ov, (size_t)total));
+          PtParams V;
+          memset(&V, 0, sizeof(V));
+          pos_view(g, V.V);
+          V.q_terms = g->q_terms.p; V.q_col = g->pt_col.p; V.q_parts = g->pt_parts.p; V.q_nparts = g->pt_nparts.p; V.q_nterms = g->q_nterms.p;
+          V.nt = nt; V.np = npw; V.token_counts = g->has_tok ? g->tok_count.p : nullptr;
+          V.cand_off = g->a3_off.p; V.cand_pre = g->ph_pre.p; V.slot0 = g0; V.n_slots = ns;
+          V.c_doc = g->ph_cdoc.p; V.c_off = g->ph_coff.p; V.c_tf = g->ph_ctf.p;
+          V.q_bits = (uint32_t* const*)g->pt_bits.p; V.counters = g->counters.p;
+          V.list = nullptr; V.n = total; V.ov_list = (unsigned long long*)g->ph_ov.p; V.ov = g->ph_ovc.p; V.scratch_cursor = g->ph_ovc.p + 2;
+          SB_CUDA(cudaMemsetAsync(g->ph_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+          const unsigned grid = (unsigned)std::min<uint64_t>(div_up(total, PT_WARPS), (uint64_t)n_sm * 16);
+          SB_TRY(timed([&]() -> int { SB_LAUNCH(k_pattern_verify, grid, PT_WARPS * 32, 0, s, V); SB_CHECK_LAUNCH(); return SB200_OK; }));
+          // candidates whose lists do not fit shared memory: one pass over global scratch (chains only shrink)
+          unsigned long long ov[4] = {0, 0, 0, 0};
+          SB_CUDA(cudaMemcpyAsync(ov, g->ph_ovc.p, sizeof(ov), cudaMemcpyDeviceToHost, s));
+          SB_CUDA(cudaStreamSynchronize(s));
+          if (ov[0]) {
+            SB_TRY(ensure(g->ph_scratch, (size_t)(ov[1] + 64)));
+            V.list = (const unsigned long long*)g->ph_ov.p; V.n = ov[0]; V.ov_list = nullptr; V.scratch = g->ph_scratch.p;
+            SB_CUDA(cudaMemsetAsync(g->ph_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+            const unsigned grid2 = (unsigned)std::min<uint64_t>(div_up(ov[0], PT_WARPS), (uint64_t)n_sm * 16);
+            SB_TRY(timed([&]() -> int { SB_LAUNCH(k_pattern_verify, grid2, PT_WARPS * 32, 0, s, V); SB_CHECK_LAUNCH(); return SB200_OK; }));
+          }
+        }
+        g0 = g1;
+      }
+    }
+    unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    SB_CUDA(cudaEventRecord(g->ev1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    if (h[2]) SB_FAIL(SB200_EFORMAT, "%llu pattern work items met inconsistent posting / position data", h[2]);
+    if (stats) {
+      stats->candidates = h[0]; stats->matches = h[1]; stats->positions_decoded = h[3]; stats->position_bytes = h[4];
+      cudaEventElapsedTime(&stats->ms, g->ev0, g->ev1); stats->kernel_ms = kms;
+    }
+    return SB200_OK;
+  }();
+  if (rc != SB200_OK) return fail_cleanup(rc);
   return SB200_OK;
 }
 
@@ -1349,7 +1643,7 @@ int sb200_phrase_topk_batch(sb200_segment* seg, const sb200_phrase_batch* batch,
 
 int sb200_multi_signal_topk_batch(const sb200_multi_signal_batch* batch, uint32_t* docs, double* totals, uint32_t* n_out,
                                   sb200_bm25_stats* stats) {
-  return run_multi(batch, docs, totals, n_out, stats);
+  return run_multi(batch, nullptr, docs, totals, n_out, stats);
 }
 int sb200_signal_topk_batch(sb200_segment* seg, const sb200_signal_batch* batch, uint32_t* docs, double* totals, uint32_t* n_out,
                             sb200_bm25_stats* stats) {
@@ -1357,6 +1651,124 @@ int sb200_signal_topk_batch(sb200_segment* seg, const sb200_signal_batch* batch,
   SB_CUDA(cudaSetDevice(seg->device));
   if (!batch || !totals) SB_FAIL(SB200_EINVAL, "NULL argument");
   return run_batch(seg, &batch->q, SB200_MODE_OR, batch, docs, nullptr, totals, n_out, stats);
+}
+
+
+int sb200_segment_attach_token_counts(sb200_segment* g, const uint64_t* counts, uint32_t max_doc) {
+  if (!g || !counts) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (max_doc != g->max_doc) SB_FAIL(SB200_EINVAL, "token counts for %u docs, the segment has %u", max_doc, g->max_doc);
+  SB_CUDA(cudaSetDevice(g->device));
+  g->has_tok = false;
+  SB_TRY(g->tok_count.alloc(std::max<uint32_t>(max_doc, 1)));
+  if (max_doc) SB_TRY(copy_in(g->tok_count.p, counts, (size_t)max_doc * 8, g->stream));
+  SB_CUDA(cudaStreamSynchronize(g->stream));
+  g->has_tok = true;
+  return SB200_OK;
+}
+
+int sb200_pattern_docsets(sb200_segment* seg, const sb200_pattern_batch* batch, sb200_docset** out, sb200_pattern_stats* stats) {
+  if (!seg) SB_FAIL(SB200_EINVAL, "NULL segment handle");
+  SB_CUDA(cudaSetDevice(seg->device));
+  return run_patterns(seg, batch, out, stats);
+}
+
+int sb200_docset_from_postings(sb200_segment* g, uint32_t term, sb200_docset** out) {
+  if (!g || !out) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (term != SB200_ABSENT_TERM && term >= g->n_terms) SB_FAIL(SB200_EINVAL, "term ordinal %u >= %u", term, g->n_terms);
+  SB_CUDA(cudaSetDevice(g->device));
+  // a one-TERM pattern takes the same path: its postings
+  const uint8_t part = SB200_PART_TERM;
+  sb200_pattern_batch b;
+  memset(&b, 0, sizeof(b));
+  b.n_patterns = 1; b.n_parts = 1; b.parts = &part; b.n_terms = 1; b.term_ords = &term;
+  return run_patterns(g, &b, out, nullptr);
+}
+
+int sb200_docset_combine(int op, const sb200_docset* const* in, uint32_t n, sb200_docset** out) {
+  if (!in || !out || n == 0) SB_FAIL(SB200_EINVAL, "NULL argument or no inputs");
+  if (op != SB200_DOCSET_AND && op != SB200_DOCSET_OR) SB_FAIL(SB200_EINVAL, "op %d", op);
+  for (uint32_t i = 0; i < n; i++) {
+    if (!in[i]) SB_FAIL(SB200_EINVAL, "input %u is NULL", i);
+    if (in[i]->max_doc != in[0]->max_doc || in[i]->device != in[0]->device)
+      SB_FAIL(SB200_EINVAL, "input %u: max_doc %u on device %d, input 0: %u on %d", i, in[i]->max_doc, in[i]->device, in[0]->max_doc, in[0]->device);
+  }
+  SB_CUDA(cudaSetDevice(in[0]->device));
+  sb200_docset* d = new (std::nothrow) sb200_docset;
+  if (!d) SB_FAIL(SB200_ENOMEM, "docset: host allocation failed");
+  d->device = in[0]->device; d->max_doc = in[0]->max_doc;
+  const uint32_t nw = std::max<uint32_t>((in[0]->max_doc + 31) / 32, 1);
+  std::vector<uint64_t> ptrs(n);
+  for (uint32_t i = 0; i < n; i++) ptrs[i] = (uint64_t)(uintptr_t)in[i]->bits.p;
+  DevBuf<uint64_t> dp;
+  int rc = d->bits.alloc(nw);
+  if (rc == SB200_OK) rc = dp.alloc(n);
+  if (rc != SB200_OK) { delete d; return rc; }
+  auto go = [&]() -> int {
+    SB_CUDA(cudaMemcpy(dp.p, ptrs.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
+    SB_LAUNCH(k_docset_combine, div_up(nw, 256), 256, 0, 0, (const uint32_t* const*)dp.p, n, op == SB200_DOCSET_AND ? 0 : 1, d->bits.p, nw);
+    SB_CHECK_LAUNCH();
+    SB_CUDA(cudaDeviceSynchronize());
+    return SB200_OK;
+  };
+  rc = go();
+  if (rc != SB200_OK) { delete d; return rc; }
+  *out = d;
+  return SB200_OK;
+}
+
+int sb200_docset_count(const sb200_docset* ds, uint64_t* count) {
+  if (!ds || !count) SB_FAIL(SB200_EINVAL, "NULL argument");
+  SB_CUDA(cudaSetDevice(ds->device));
+  DevBuf<unsigned long long> c;
+  SB_TRY(c.alloc(1));
+  SB_CUDA(cudaMemset(c.p, 0, 8));
+  const uint32_t nw = (ds->max_doc + 31) / 32;
+  if (nw) {
+    SB_LAUNCH(k_docset_count, std::min<unsigned>(div_up(nw, 256), 1024u), 256, 0, 0, ds->bits.p, nw, c.p);
+    SB_CHECK_LAUNCH();
+  }
+  unsigned long long h = 0;
+  SB_CUDA(cudaMemcpy(&h, c.p, 8, cudaMemcpyDeviceToHost));
+  *count = h;
+  return SB200_OK;
+}
+
+// an inspection read-back: the bitmap crosses to the host and is expanded there
+int sb200_docset_read(const sb200_docset* ds, uint32_t* docs, uint64_t cap, uint64_t* total) {
+  if (!ds || !total || (cap && !docs)) SB_FAIL(SB200_EINVAL, "NULL argument");
+  SB_CUDA(cudaSetDevice(ds->device));
+  const uint32_t nw = (ds->max_doc + 31) / 32;
+  std::vector<uint32_t> w(nw);
+  if (nw) SB_CUDA(cudaMemcpy(w.data(), ds->bits.p, (size_t)nw * 4, cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> out;
+  uint64_t n = 0;
+  for (uint32_t i = 0; i < nw; i++)
+    for (uint32_t x = w[i]; x; x &= x - 1) {
+      if (n < cap) out.push_back(i * 32u + (uint32_t)__builtin_ctz(x));
+      n++;
+    }
+  if (!out.empty()) SB_CUDA(cudaMemcpy(docs, out.data(), out.size() * 4, cudaMemcpyDefault));
+  *total = n;
+  return SB200_OK;
+}
+
+int sb200_docset_info(const sb200_docset* ds, uint32_t* max_doc, int* device) {
+  if (!ds) SB_FAIL(SB200_EINVAL, "NULL docset handle");
+  if (max_doc) *max_doc = ds->max_doc;
+  if (device) *device = ds->device;
+  return SB200_OK;
+}
+
+void sb200_docset_destroy(sb200_docset* ds) {
+  if (!ds) return;
+  cudaSetDevice(ds->device);
+  delete ds;
+}
+
+int sb200_multi_signal_topk_batch_optic(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, uint32_t* docs,
+                                        double* totals, uint32_t* n_out, sb200_bm25_stats* stats) {
+  if (!optic) SB_FAIL(SB200_EINVAL, "NULL optic batch");
+  return run_multi(batch, optic, docs, totals, n_out, stats);
 }
 
 }  // extern "C"

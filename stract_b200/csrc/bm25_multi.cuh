@@ -20,6 +20,9 @@
 // boost beside it), placed behind the text slots by the host.  Rule slots are probed, never enumerated on their own: a
 // document owned by a rule slot is in no text slot and is skipped.  Matching rules add to `boost` or `downrank` in rule
 // order and the total is multiplied by  downrank > boost ? 1/(1 + (downrank - boost)) : boost - downrank + 1.
+// OPTIC = true (sb200_multi_signal_topk_batch_optic): rules are device docsets (bm25_pattern.cuh) instead of slots.  A
+// candidate in the query's exclude bitmap or outside its require bitmap is dropped before scoring (the MustNot / Must filters
+// of Discard and DiscardNonMatching); the rules' bits feed the same down / up sums in rule order and the same factor.
 #pragma once
 
 namespace sb200 {
@@ -45,14 +48,20 @@ struct MParams {
   const double* sig; uint32_t n_cols;
   uint64_t* g_khi; uint32_t* g_klo;
   uint32_t* o_docs; double* o_totals; uint32_t* o_n; unsigned long long* counters;
+  // optic docsets (k_sig_multi<TMAX, true>), per caller query index (q_orig): rules, boosts and the two filters
+  const uint32_t* const* d_bits;   // [n_docsets] bitmaps
+  const uint32_t* d_nrules; const uint32_t* d_rule; const double* d_boost; uint32_t d_max_rules;
+  const uint32_t* d_exclude; const uint32_t* d_require;   // SB200_NO_DOCSET: none
 };
+
+__device__ __forceinline__ bool m_in(const uint32_t* bits, uint32_t d) { return (__ldg(bits + (d >> 5)) >> (d & 31u)) & 1u; }
 
 template <int TMAX>
 __host__ __device__ constexpr size_t m_warp_smem() { return (size_t)TMAX * 128 * 8 + (size_t)TMAX * 16 * 4 + (size_t)TMAX * sizeof(OTerm) + (size_t)TMAX * 8 + 48 * 4; }
 template <int TMAX>
 __host__ __device__ constexpr size_t m_cta_smem() { return M_MAX_FIELDS * 256 * 4 + M_MAX_OPS * sizeof(MOp) + WQ * m_warp_smem<TMAX>(); }
 
-template <int TMAX>
+template <int TMAX, bool OPTIC = false>
 __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
   SB_DYN_SMEM(smem_raw);
   float* s_cache = (float*)smem_raw;                                   // [M_MAX_FIELDS][256]
@@ -82,6 +91,15 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
   const uint32_t T = min(P.q_nslots[q], (uint32_t)TMAX);
   uint64_t* khi = P.g_khi + (size_t)item * P.cap; uint32_t* klo = P.g_klo + (size_t)item * P.cap;
   const bool ranged = lo_doc > 0 || hi_doc != 0xFFFFFFFFu;
+  const uint32_t* o_ex = nullptr; const uint32_t* o_rq = nullptr;
+  uint32_t o_nr = 0, o_q = 0;
+  if constexpr (OPTIC) {
+    o_q = P.q_orig ? P.q_orig[q] : q;
+    const uint32_t ex = P.d_exclude ? P.d_exclude[o_q] : SB200_NO_DOCSET, rq = P.d_require ? P.d_require[o_q] : SB200_NO_DOCSET;
+    if (ex != SB200_NO_DOCSET) o_ex = P.d_bits[ex];
+    if (rq != SB200_NO_DOCSET) o_rq = P.d_bits[rq];
+    o_nr = P.d_nrules ? P.d_nrules[o_q] : 0u;
+  }
 
   // ---- cursors: lane t owns slot t
   uint32_t my_pos = 0, my_len = 0, my_last = 0, my_cur = 0, my_prev = 0;
@@ -209,6 +227,10 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
       }
       if (!owner) continue;
       if (s_fld[i] & 0x80u) continue;   // only rule docsets hold this doc: not a candidate
+      if constexpr (OPTIC) {
+        if (o_ex && m_in(o_ex, d)) continue;    // Discard rules, blocked hosts
+        if (o_rq && !m_in(o_rq, d)) continue;   // DiscardNonMatching
+      }
       my_docs++;
       uint32_t fid[M_MAX_FIELDS];
 #pragma unroll
@@ -276,6 +298,19 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
         }
         const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
         total = __dmul_rn(total, factor);
+      }
+      if constexpr (OPTIC) {
+        if (o_nr) {   // SignalComputer::boosts over the rule docsets, in rule order
+          double down = 0.0, up = 0.0;
+          for (uint32_t r = 0; r < o_nr; r++) {
+            const size_t at = (size_t)o_q * P.d_max_rules + r;
+            if (!m_in(P.d_bits[P.d_rule[at]], d)) continue;
+            const double b = P.d_boost[at];
+            if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
+          }
+          const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
+          total = __dmul_rn(total, factor);
+        }
       }
       const uint64_t kh = ord_f64(total);
       const uint32_t kl = ~d;

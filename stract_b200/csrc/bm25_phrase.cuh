@@ -207,7 +207,9 @@ struct PhCandParams {
   uint32_t* c_doc; uint64_t* c_off; uint32_t* c_tf;   // [entry], [entry][nt], [entry][nt]
 };
 
-// dynamic shared memory: [A3_WARPS][nt][128] u64 position offsets, then [A3_WARPS][nt][128] u32 tfs
+// dynamic shared memory: [A3_WARPS][nt][128] u64 position offsets, then [A3_WARPS][nt][128] u32 tfs.  MIN_T: rows with
+// fewer terms produce nothing (phrases: 2; optic patterns, bm25_pattern.cuh: 1, every posting of a one-term row is a candidate)
+template <uint32_t MIN_T>
 __global__ void __launch_bounds__(A3_WARPS * 32) k_phrase_cand(const PhCandParams C) {
   SB_DYN_SMEM(smem_raw);
   __shared__ __align__(16) uint32_t s_docs[A3_WARPS][128];
@@ -226,7 +228,7 @@ __global__ void __launch_bounds__(A3_WARPS * 32) k_phrase_cand(const PhCandParam
   uint32_t* sd = s_docs[warp]; uint32_t* stf = s_tfs[warp]; uint32_t* spre = s_pre[warp]; uint32_t* cur = s_cur[warp];
   if (lane < MAXT) cur[lane] = 0;
   __syncwarp();
-  if (T < 2) return;
+  if (T < MIN_T) return;
   const A3Term tA = a3_load_term(P, q, 0);
   unsigned long long n_blocks = 0, n_hits = 0;
   bool watchdog = false, bad_doc = false;
