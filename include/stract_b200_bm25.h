@@ -338,6 +338,57 @@ typedef struct {
 SB200_API int sb200_multi_signal_topk_batch_optic(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, uint32_t* docs,
                                                   double* totals, uint32_t* n_out, sb200_bm25_stats* stats);
 
+/* ---- the recall docset of Stract's query plan (core/src/query/plan/, Query::parse in core/src/query/mod.rs:106-122) ----------
+ * A query's plan, compiled to a tantivy BooleanQuery and evaluated with scoring disabled, is a post-order program of nodes:
+ *   SB200_PLAN_TERM    segment, arg = term ordinal or SB200_ABSENT_TERM (an empty TermScorer): the term's postings
+ *   SB200_PLAN_PHRASE  segment, arg = a row of the phrase table (terms and offsets as in sb200_phrase_batch, slop per row):
+ *                      PhraseScorer::phrase_exists (scoring is disabled); a row with an SB200_ABSENT_TERM matches nothing.  The
+ *                      segment needs positions (SB200_RECORD_FREQS_POSITIONS and sb200_segment_attach_positions).
+ *   SB200_PLAN_EMPTY   BooleanQuery::new(vec![]): matches nothing
+ *   SB200_PLAN_BOOL    the n_children nodes before it (each a subtree) are its clauses, with their `occur`; BooleanWeight
+ *                      (boolean_weight.rs:107-180): no clauses -> empty; one MustNot clause alone -> empty; one other clause ->
+ *                      that clause; otherwise the Must intersection (Should clauses are ignored when a Must exists) or else the
+ *                      Should union, minus the MustNot union; neither Must nor Should -> empty.
+ * `occur` is the node's occur in its parent (SB200_PLAN_MUST / SHOULD / MUST_NOT); the root's is ignored.  Query q owns nodes
+ * [node_off[q], node_off[q + 1]), at most SB200_PLAN_MAX_NODES, and the program must leave exactly one value.  Plan segments are
+ * their own array: leaves span fields that are not signal fields (UrlForSiteOperator, Links, compound fields).  Every segment
+ * must have the same max_doc and device (fields of one tantivy segment).  Malformed programs, bad indices and mismatched
+ * segments are SB200_EINVAL. */
+#define SB200_PLAN_TERM 0u
+#define SB200_PLAN_PHRASE 1u
+#define SB200_PLAN_EMPTY 2u
+#define SB200_PLAN_BOOL 3u
+#define SB200_PLAN_MUST 0u
+#define SB200_PLAN_SHOULD 1u
+#define SB200_PLAN_MUST_NOT 2u
+#define SB200_PLAN_MAX_NODES 256
+typedef struct { uint8_t kind, occur; uint16_t n_children; uint32_t segment; uint32_t arg; uint32_t _pad; } sb200_plan_node;
+typedef struct {
+  uint32_t n_queries, n_segments;
+  sb200_segment* const* segments;   /* [n_segments] */
+  const uint32_t* node_off;         /* [n_queries + 1] */
+  const sb200_plan_node* nodes;     /* [node_off[n_queries]] */
+  uint32_t n_phrases, phrase_terms; /* rows of the phrase table, row width (2..SB200_MAX_QUERY_TERMS, SB200_NO_TERM pads a row's end) */
+  const uint32_t* phrase_ords;      /* [n_phrases * phrase_terms] ordinals or SB200_ABSENT_TERM; NULL when no node is a PHRASE */
+  const uint32_t* phrase_offsets;   /* [n_phrases * phrase_terms] position offset of each term; NULL = 0, 1, 2, ... */
+  const uint32_t* phrase_slop;      /* [n_phrases]; NULL = 0 */
+} sb200_recall_plan_batch;
+/* cover: candidates decoded (a superset of each query's docset, see DESIGN.md), docs: documents in the docsets, groups: query
+ * groups the candidate budget split the batch into; ms: the whole call, kernel_ms: the launches (CUDA events). */
+typedef struct { uint64_t cover, docs; uint32_t groups, _pad; float ms, kernel_ms; } sb200_plan_stats;
+/* Every query's plan docset: counts[q] documents, the first min(cap, counts[q]) of them ascending in docs[q * cap ..].
+ * docs may be NULL when cap == 0.  counts and docs may be host or device memory. */
+SB200_API int sb200_recall_plan_docs(const sb200_recall_plan_batch* plan, uint64_t* counts, uint32_t* docs, uint64_t cap,
+                                     sb200_plan_stats* stats);
+/* The multi-field recall stage (sb200_multi_signal_topk_batch, same slots, ops and outputs) over exactly each query's plan
+ * docset, after the optic filters of sb200_multi_signal_topk_batch_optic (optic nullable): BooleanQuery[(Must, plan), optic
+ * clauses...] (query/mod.rs:133-137).  A document that no slot holds is scored with every text signal 0.  The plan batch
+ * must have as many queries as the signal batch and the segments the signal fields' max_doc and device.
+ * stats->docs_scored counts the documents scored, kernel_ms covers both stages. */
+SB200_API int sb200_multi_signal_topk_batch_plan(const sb200_multi_signal_batch* batch, const sb200_recall_plan_batch* plan,
+                                                 const sb200_optic_batch* optic, uint32_t* docs, double* totals, uint32_t* n_out,
+                                                 sb200_bm25_stats* stats);
+
 /* idf(doc_freq, doc_count) = ln(1 + (N - n + 0.5) / (n + 0.5)) in f32 (tantivy/src/query/bm25.rs:52-56,
  * core/src/ranking/bm25.rs:23-27) for an array of doc_freqs; tantivy_weight != 0 returns Bm25Weight.weight = idf * (1 + K1). */
 SB200_API int sb200_bm25_idf(const uint32_t* doc_freq, uint64_t n, uint64_t doc_count, int tantivy_weight, float* out);

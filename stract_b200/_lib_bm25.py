@@ -66,6 +66,22 @@ class PatternStats(C.Structure):
                 ("ms", C.c_float), ("kernel_ms", C.c_float)]
 
 
+class PlanNode(C.Structure):
+    _fields_ = [("kind", C.c_uint8), ("occur", C.c_uint8), ("n_children", C.c_uint16), ("segment", C.c_uint32), ("arg", C.c_uint32),
+                ("_pad", C.c_uint32)]
+
+
+class RecallPlanBatch(C.Structure):
+    _fields_ = [("n_queries", C.c_uint32), ("n_segments", C.c_uint32), ("segments", C.c_void_p), ("node_off", C.c_void_p),
+                ("nodes", C.c_void_p), ("n_phrases", C.c_uint32), ("phrase_terms", C.c_uint32), ("phrase_ords", C.c_void_p),
+                ("phrase_offsets", C.c_void_p), ("phrase_slop", C.c_void_p)]
+
+
+class PlanStats(C.Structure):
+    _fields_ = [("cover", C.c_uint64), ("docs", C.c_uint64), ("groups", C.c_uint32), ("_pad", C.c_uint32), ("ms", C.c_float),
+                ("kernel_ms", C.c_float)]
+
+
 class OpticBatch(C.Structure):
     _fields_ = [("n_docsets", C.c_uint32), ("max_rules", C.c_uint32), ("docsets", C.c_void_p), ("n_rules", C.c_void_p),
                 ("rule_docset", C.c_void_p), ("rule_boost", C.c_void_p), ("exclude", C.c_void_p), ("require", C.c_void_p)]
@@ -104,3 +120,6 @@ def proto(L, f):
     f("sb200_docset_info", i32, vp, C.POINTER(u32), C.POINTER(i32))
     f("sb200_docset_destroy", None, vp)
     f("sb200_multi_signal_topk_batch_optic", i32, C.POINTER(MultiSignalBatch), C.POINTER(OpticBatch), vp, vp, vp, C.POINTER(Bm25Stats))
+    f("sb200_recall_plan_docs", i32, C.POINTER(RecallPlanBatch), vp, vp, u64, C.POINTER(PlanStats))
+    f("sb200_multi_signal_topk_batch_plan", i32, C.POINTER(MultiSignalBatch), C.POINTER(RecallPlanBatch), C.POINTER(OpticBatch), vp, vp, vp,
+      C.POINTER(Bm25Stats))

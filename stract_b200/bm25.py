@@ -840,14 +840,16 @@ class MultiFieldSignalComputer:
                 c = self.coefficient(name, coef)
         return c
 
-    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None, optic=None):
+    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None, optic=None, plan=None):
         """slot_field / slot_term [n_queries, n_slots]: field index into `self.names` (TextFieldEnum order; 0xFF pads) and the term's ordinal in that
         field's reader (NO_TERM = the segment does not hold it).  idf comes from the field's own doc_freq
         (MultiBm25Weight::for_terms), the Bm25F idf from `doc_freq_all_body` [n_queries, n_slots] (WeightCache: the AllBody
         doc_freq of the token), defaulting to the field's own.  Optic rules: a slot with field | 0x80 is the docset of a rule,
         `slot_boost` [n_queries, n_slots] holds its boost (negative = downrank): SignalComputer::boosts (mod.rs:471-497).
         `optic` (OpticTables, e.g. from stract_b200.optic.compile_optics): optic rules as device docsets, with the Discard /
-        DiscardNonMatching filters (sb200_multi_signal_topk_batch_optic); None keeps sb200_multi_signal_topk_batch."""
+        DiscardNonMatching filters (sb200_multi_signal_topk_batch_optic); None keeps sb200_multi_signal_topk_batch.
+        `plan` (RecallPlan, e.g. from stract_b200.query_plan.compile_plans): the candidates are each query's plan docset instead
+        of the union of its text slots (sb200_multi_signal_topk_batch_plan); None keeps the union."""
         sf = np.ascontiguousarray(slot_field, np.uint8); st = np.ascontiguousarray(slot_term, np.uint32)
         nq, ns = sf.shape
         idf1 = np.zeros((nq, ns), np.float32); idf2 = np.zeros((nq, ns), np.float32)
@@ -882,9 +884,10 @@ class MultiFieldSignalComputer:
         sbst = None if slot_boost is None else np.ascontiguousarray(slot_boost, np.float64)
         mb.slot_boost = _p(sbst)
         stt = B.Bm25Stats()
-        if optic is None:
+        ob = None
+        if optic is None and plan is None:
             check(self._L.sb200_multi_signal_topk_batch(C.byref(mb), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
-        else:
+        elif optic is not None:
             if len(optic.rules) != nq:
                 raise ValueError(f"optic tables for {len(optic.rules)} queries, batch has {nq}")
             mr = max([len(r) for r in optic.rules] + [1])
@@ -899,8 +902,86 @@ class MultiFieldSignalComputer:
             ob = B.OpticBatch()
             ob.n_docsets, ob.max_rules, ob.docsets = len(optic.docsets), mr, C.cast(darr, C.c_void_p)
             ob.n_rules, ob.rule_docset, ob.rule_boost, ob.exclude, ob.require = _p(nr), _p(rd), _p(rb), _p(ex), _p(rq)
-            check(self._L.sb200_multi_signal_topk_batch_optic(C.byref(mb), C.byref(ob), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+            if plan is None:
+                check(self._L.sb200_multi_signal_topk_batch_optic(C.byref(mb), C.byref(ob), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+        if plan is not None:
+            if plan.n_queries != nq:
+                raise ValueError(f"plan for {plan.n_queries} queries, batch has {nq}")
+            pb, keep = plan._batch()
+            check(self._L.sb200_multi_signal_topk_batch_plan(C.byref(mb), C.byref(pb), None if ob is None else C.byref(ob), _p(docs),
+                                                             _p(totals), _p(n_out), C.byref(stt)))
         self.last_inputs = dict(idf=idf1, idf_f=idf2, caches=caches)
         if return_stats:
             return docs, totals, n_out, {k_: getattr(stt, k_) for k_, _ in B.Bm25Stats._fields_ if not k_.startswith("_")}
         return docs, totals, n_out
+
+
+# ---------------------------------------------------------------------------------------------- query-plan recall docset ----
+PLAN_TERM, PLAN_PHRASE, PLAN_EMPTY, PLAN_BOOL = 0, 1, 2, 3
+PLAN_MUST, PLAN_SHOULD, PLAN_MUST_NOT = 0, 1, 2
+PLAN_MAX_NODES = 256
+
+
+class RecallPlan:
+    """A batch of compiled query plans (sb200_recall_plan_batch): `segments` the plan's fields (SegmentReaders of one tantivy
+    segment, signal fields or not), `programs[q]` the post-order node list of query q, each node a tuple
+    (kind, occur, n_children, segment index, arg) -- arg: the term's ordinal or ABSENT_TERM for PLAN_TERM, a row of `phrases`
+    for PLAN_PHRASE.  `phrases`: rows (term ordinals in offset order, offsets or None for 0, 1, 2, ..., slop)."""
+
+    def __init__(self, segments, programs, phrases=()):
+        self.segments = list(segments)
+        self.programs = [list(p) for p in programs]
+        self.phrases = [(list(t), None if o is None else list(o), int(sl)) for t, o, sl in phrases]
+        self.n_queries = len(self.programs)
+
+    def _batch(self):
+        nodes = (B.PlanNode * max(sum(len(p) for p in self.programs), 1))()
+        off = np.zeros(self.n_queries + 1, np.uint32)
+        i = 0
+        for q, prog in enumerate(self.programs):
+            for kind, occur, nc, seg, arg in prog:
+                n = nodes[i]
+                n.kind, n.occur, n.n_children, n.segment, n.arg = kind, occur, nc, seg, arg
+                i += 1
+            off[q + 1] = i
+        segs = (C.c_void_p * len(self.segments))(*[s._h.value if hasattr(s._h, "value") else s._h for s in self.segments])
+        pb = B.RecallPlanBatch()
+        pb.n_queries, pb.n_segments = self.n_queries, len(self.segments)
+        pb.segments, pb.node_off, pb.nodes = C.cast(segs, C.c_void_p), _p(off), C.cast(nodes, C.c_void_p)
+        keep = [nodes, off, segs]
+        if self.phrases:
+            width = max(len(t) for t, _, _ in self.phrases)
+            if width > MAX_QUERY_TERMS:
+                raise ValueError(f"a phrase of {width} terms (at most {MAX_QUERY_TERMS})")
+            width = max(width, 2)
+            ords = np.full((len(self.phrases), width), NO_TERM, np.uint32); offs = np.zeros((len(self.phrases), width), np.uint32)
+            slop = np.zeros(len(self.phrases), np.uint32)
+            for r, (t, o, sl) in enumerate(self.phrases):
+                ords[r, :len(t)] = t
+                offs[r, :len(t)] = np.arange(len(t)) if o is None else o
+                slop[r] = sl
+            pb.n_phrases, pb.phrase_terms = len(self.phrases), width
+            pb.phrase_ords, pb.phrase_offsets, pb.phrase_slop = _p(ords), _p(offs), _p(slop)
+            keep += [ords, offs, slop]
+        return pb, keep
+
+
+def recall_plan_docs(plan, return_stats=False):
+    """Every query's plan docset as an ascending uint32 array (sb200_recall_plan_docs).  The docset stage runs once when every
+    docset fits `cap` documents, and once more with the largest count otherwise."""
+    pb, keep = plan._batch()
+    L = plan.segments[0]._L
+    nq = plan.n_queries
+    counts = np.zeros(nq, np.uint64)
+    st = B.PlanStats()
+    cap = 4096
+    docs = np.zeros((max(nq, 1), cap), np.uint32)
+    check(L.sb200_recall_plan_docs(C.byref(pb), _p(counts), _p(docs), cap, C.byref(st)))
+    if nq and int(counts.max()) > cap:
+        cap = int(counts.max())
+        docs = np.zeros((nq, cap), np.uint32)
+        check(L.sb200_recall_plan_docs(C.byref(pb), _p(counts), _p(docs), cap, C.byref(st)))
+    out = [docs[q, :int(counts[q])].copy() for q in range(nq)]
+    if return_stats:
+        return out, {k_: getattr(st, k_) for k_, _ in B.PlanStats._fields_ if not k_.startswith("_")}
+    return out

@@ -22,6 +22,7 @@
 //   phrases              k_phrase_cand + k_phrase_verify + k_and3_select (bm25_phrase.cuh).
 //   optic pattern docsets k_phrase_cand + k_pattern_verify and word kernels (bm25_pattern.cuh); k_sig_multi<TMAX, true>
 //                        consumes them in the recall stage.
+//   query-plan docsets   k_plan_cover + CUB sort + k_plan_eval + CUB select (bm25_plan.cuh); k_plan_recall scores them.
 // A query of the walk kernels much larger than the batch average is cut into doc-range work items (plan_items);
 // k_merge_topk merges their partial top-k lists.  Keys are (order-preserving score bits, ~doc), so the result order
 // is the reference's (score desc, doc asc) total order.
@@ -103,6 +104,10 @@ struct sb200_segment {
   // scratch of the pattern path and of the optic recall stage (the latter in the first field's handle)
   sb200::DevBuf<uint32_t> pt_col, pt_nparts; sb200::DevBuf<uint8_t> pt_parts; sb200::DevBuf<uint64_t> pt_bits;
   sb200::DevBuf<uint64_t> o_bits; sb200::DevBuf<uint32_t> o_nrules, o_rule, o_exclude, o_require; sb200::DevBuf<double> o_boost;
+  // scratch of the plan docset stage (bm25_plan.cuh; in the first plan segment's handle)
+  sb200::DevBuf<uint8_t> pl_segs, pl_nodes, pl_cover, pl_keep, pl_tmp;
+  sb200::DevBuf<uint64_t> pl_keys, pl_keys2, pl_beg, pl_cnt;
+  sb200::DevBuf<uint32_t> pl_off, pl_units, pl_ph_off, pl_ph_docs;
 };
 
 struct sb200_docset {
@@ -268,6 +273,9 @@ static int launch_topk_warp(const WParams& P, cudaStream_t s) {
 #include "bm25_wand.cuh"
 #include "bm25_phrase.cuh"
 #include "bm25_pattern.cuh"
+#include "bm25_plan.cuh"
+#include <chrono>
+#include <functional>
 namespace sb200 {
 
 static void seg_view(const sb200_segment* g, SegView& S) {
@@ -316,8 +324,21 @@ static int launch_multi(const MParams& P, cudaStream_t s) {
   return SB200_OK;
 }
 
+typedef std::function<int(uint32_t g0, uint32_t g1, const uint64_t* keys, const uint64_t* q_beg, const std::vector<uint64_t>& h_beg)> PlanEmit;
+static int run_plan(const sb200_recall_plan_batch* pb, PlanEmit emit, sb200_plan_stats* stats);
+template <int TMAX>
+static int launch_plan_recall(const PlanRecallParams& R, cudaStream_t s) {
+  const size_t sm = pl_cta_smem<TMAX>();
+  static bool configured = false;
+  if (!configured) { SB_CUDA(cudaFuncSetAttribute(k_plan_recall<TMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); configured = true; }
+  SB_LAUNCH(k_plan_recall<TMAX>, div_up(R.M.n_queries, WQ), WQ * 32, sm, s, R);
+  SB_CHECK_LAUNCH();
+  return SB200_OK;
+}
+
+// pb != NULL: the candidates are each query's plan docset (run_plan) instead of the union of its text slots
 static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch* ob, uint32_t* docs, double* totals, uint32_t* n_out,
-                     sb200_bm25_stats* stats) {
+                     sb200_bm25_stats* stats, const sb200_recall_plan_batch* pb = nullptr) {
   if (!b || !b->fields || !b->ops || !b->slot_field || !b->slot_term || !b->slot_idf || !b->slot_idf_f || !docs || !totals || !n_out)
     SB_FAIL(SB200_EINVAL, "NULL argument");
   const uint32_t nq = b->n_queries, SM = b->n_slots, k = b->k, NF = b->n_fields, NO = b->n_ops;
@@ -345,6 +366,14 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     }
   }
   if (n_cols && b->signals->max_doc < g->max_doc) SB_FAIL(SB200_EINVAL, "signal table covers %u docs, segment has %u", b->signals->max_doc, g->max_doc);
+  if (pb) {
+    if (pb->n_queries != nq) SB_FAIL(SB200_EINVAL, "plan batch has %u queries, signal batch %u", pb->n_queries, nq);
+    if (!pb->segments || pb->n_segments == 0) SB_FAIL(SB200_EINVAL, "plan batch without segments");
+    for (uint32_t i = 0; i < pb->n_segments; i++) {
+      const sb200_segment* x = pb->segments[i];
+      if (!x || x->device != g->device || x->max_doc != g->max_doc) SB_FAIL(SB200_EINVAL, "plan segment %u is not a field of the signal fields' segment (device / max_doc differ)", i);
+    }
+  }
   if (ob) {   // optic docsets: shapes, indices, devices; rule slots and docset rules never share a query
     if (ob->n_docsets && !ob->docsets) SB_FAIL(SB200_EINVAL, "optic: NULL docsets");
     if (ob->n_rules && (!ob->rule_docset || !ob->rule_boost)) SB_FAIL(SB200_EINVAL, "optic: NULL rule_docset / rule_boost");
@@ -385,7 +414,7 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     }
     postings += work[q];
   }
-  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t c) { return work[a] > work[c]; });
+  if (!pb) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t c) { return work[a] > work[c]; });
   for (uint32_t slot = 0; slot < nq; slot++) {
     const uint32_t q = order[slot];
     uint32_t c = 0;
@@ -400,8 +429,8 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
       }
     ns[slot] = c; work_sorted[slot] = work[q];
   }
-  ItemPlan pl;
-  plan_items(work_sorted, order, k, g->max_doc, true, pl);
+  ItemPlan pl;   // the plan path has its own work items (one per query, k_plan_recall) and candidate buffers
+  if (!pb) plan_items(work_sorted, order, k, g->max_doc, true, pl);
   const uint32_t n_items = (uint32_t)pl.q.size();
   const size_t n_slots_out = (size_t)nq + pl.extra;
   uint32_t cap = 1024; while (cap < k + SM * 128u) cap <<= 1;
@@ -470,6 +499,56 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     SB_CUDA(cudaMemcpyAsync(g->o_boost.p, rb.data(), rb.size() * 8, cudaMemcpyHostToDevice, s));
     P.d_bits = (const uint32_t* const*)g->o_bits.p; P.d_nrules = g->o_nrules.p; P.d_rule = g->o_rule.p; P.d_boost = g->o_boost.p;
     P.d_max_rules = MR; P.d_exclude = g->o_exclude.p; P.d_require = g->o_require.p;
+  }
+  if (pb) {   // the plan docset group by group; each group's recall runs on this stream once its docset is complete
+    SB_CUDA(cudaStreamSynchronize(s));
+    uint32_t rcap = 1024; while (rcap < k + 32) rcap <<= 1;
+    float kms = 0.0f; unsigned long long scored = 0;
+    sb200_plan_stats ps;
+    bool restored = false;
+    auto emit = [&](uint32_t g0, uint32_t g1, const uint64_t* keys, const uint64_t* q_beg, const std::vector<uint64_t>&) -> int {
+      const uint32_t n = g1 - g0;
+      if (!restored) {
+        // phrase leaves on this handle's field ran the phrase path on it, which reuses (and may have regrown) its term, weight,
+        // count and counter scratch: upload the slots again and point the parameters at the current buffers
+        SB_TRY(ensure(g->q_terms, st.size())); SB_TRY(ensure(g->q_weights, w1.size())); SB_TRY(ensure(g->q_nterms, ns.size())); SB_TRY(ensure(g->counters, 4));
+        SB_CUDA(cudaMemcpyAsync(g->q_terms.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));
+        SB_CUDA(cudaMemcpyAsync(g->q_weights.p, w1.data(), w1.size() * 4, cudaMemcpyHostToDevice, s));
+        SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, ns.data(), ns.size() * 4, cudaMemcpyHostToDevice, s));
+        SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 4 * sizeof(unsigned long long), s));
+        P.q_slot_term = g->q_terms.p; P.q_idf = g->q_weights.p; P.q_nslots = g->q_nterms.p; P.counters = g->counters.p;
+        restored = true;
+      }
+      SB_TRY(ensure(g->g_khi, (size_t)n * rcap)); SB_TRY(ensure(g->g_klo, (size_t)n * rcap));
+      PlanRecallParams R;
+      R.M = P;
+      R.M.q_slot_field = P.q_slot_field + (size_t)g0 * SM; R.M.q_slot_term = P.q_slot_term + (size_t)g0 * SM;
+      R.M.q_idf = P.q_idf + (size_t)g0 * SM; R.M.q_idf_f = P.q_idf_f + (size_t)g0 * SM; R.M.q_nslots = P.q_nslots + g0;
+      if (P.q_boost) R.M.q_boost = P.q_boost + (size_t)g0 * SM;
+      R.M.q_orig = P.q_orig + g0; R.M.n_queries = n; R.M.cap = rcap; R.M.g_khi = g->g_khi.p; R.M.g_klo = g->g_klo.p;
+      R.keys = keys; R.q_beg = q_beg;
+      SB_CUDA(cudaEventRecord(g->evk0, s));
+      if (SM <= 8) SB_TRY(launch_plan_recall<8>(R, s)); else SB_TRY(launch_plan_recall<16>(R, s));
+      SB_CUDA(cudaEventRecord(g->evk1, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+      return SB200_OK;
+    };
+    SB_TRY(run_plan(pb, emit, &ps));
+    SB_CUDA(cudaMemcpyAsync(docs, g->o_docs.p, (size_t)nq * k * 4, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemcpyAsync(totals, g->o_totals.p, (size_t)nq * k * 8, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemcpyAsync(n_out, g->o_n.p, (size_t)nq * 4, cudaMemcpyDefault, s));
+    unsigned long long h[4] = {0, 0, 0, 0};
+    SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    SB_CUDA(cudaEventRecord(g->ev1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    if (h[2]) SB_FAIL(SB200_EFORMAT, "%llu queries met inconsistent posting data in the plan recall", h[2]);
+    scored = h[0];
+    if (stats) {
+      float ms = 0; cudaEventElapsedTime(&ms, g->ev0, g->ev1);
+      stats->postings_scored = postings; stats->docs_scored = scored; stats->blocks_decoded = 0; stats->ms = ms; stats->kernel_ms = kms + ps.kernel_ms;
+    }
+    return SB200_OK;
   }
   SB_CUDA(cudaEventRecord(g->evk0, s));
   if (ob) { if (SM <= 8) SB_TRY((launch_multi<8, true>(P, s))); else SB_TRY((launch_multi<16, true>(P, s))); }
@@ -784,39 +863,27 @@ static void pos_view(const sb200_segment* g, PosView& V) {
   V.count = g->pos_count.p; V.first = g->pos_first.p; V.nblk = g->pos_nblk.p; V.b_off = g->pos_b_off.p; V.b_w = g->pos_b_w.p;
 }
 
-// Phrase batch (bm25_phrase.cuh).  Host planning mirrors PhraseWeight::phrase_scorer: a term the segment does not hold empties
-// the phrase; the others are put in Intersection order (stable sort by doc_freq, intersection.rs:69-81) with their shift
-// max_offset - offset.  Queries are processed in groups whose candidate records fit a memory budget.
-static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* docs, float* scores, uint32_t* n_out, sb200_phrase_stats* stats) {
-  NvtxRange nvtx("sb200 phrase top-k batch");
-  cudaStream_t s = g->stream;
-  if (!b || !b->term_ords || !docs || !scores || !n_out) SB_FAIL(SB200_EINVAL, "NULL argument");
-  if (b->scoring && (!b->weights || !b->tf_cache256)) SB_FAIL(SB200_EINVAL, "scoring needs weights and tf_cache256");
-  if (g->record != SB200_RECORD_FREQS_POSITIONS) SB_FAIL(SB200_EINVAL, "phrase query on a field without positions (record option %d)", g->record);
-  if (!g->has_pos) SB_FAIL(SB200_EINVAL, "phrase query: no positions attached to the segment (sb200_segment_attach_positions)");
-  const uint32_t nq = b->n_queries, nt = b->n_terms, k = b->k;
-  if (nt < 2 || nt > MAXT) SB_FAIL(SB200_ERANGE, "n_terms %u outside [2,%d]", nt, MAXT);
-  if (k == 0 || k > SB200_MAX_K) SB_FAIL(SB200_ERANGE, "k %u outside [1,%d]", k, SB200_MAX_K);
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (nq == 0) return SB200_OK;
-  std::vector<uint32_t> terms((size_t)nq * nt, 0), shift((size_t)nq * nt, 0), nterms(nq, 0), slop(nq, 0);
-  std::vector<float> weight(nq, 0.0f);
+// Host planning of phrase rows, as PhraseWeight::phrase_scorer: a term the segment does not hold empties the phrase (its row
+// keeps 0 terms); the others are put in Intersection order (stable sort by doc_freq, intersection.rs:69-81) with their shift
+// max_offset - offset.
+static int phrase_rows(const sb200_segment* g, uint32_t nq, uint32_t nt, const uint32_t* ords_in, const uint32_t* offsets, const uint32_t* slops,
+                       std::vector<uint32_t>& terms, std::vector<uint32_t>& shift, std::vector<uint32_t>& nterms, std::vector<uint32_t>& slop) {
+  terms.assign((size_t)nq * nt, 0); shift.assign((size_t)nq * nt, 0); nterms.assign(nq, 0); slop.assign(nq, 0);
   for (uint32_t q = 0; q < nq; q++) {
     uint32_t ords[MAXT], offs[MAXT], c = 0;
     bool absent = false;
     for (uint32_t t = 0; t < nt; t++) {
-      const uint32_t ord = b->term_ords[(size_t)q * nt + t];
+      const uint32_t ord = ords_in[(size_t)q * nt + t];
       if (ord == SB200_NO_TERM) {
-        for (uint32_t u = t; u < nt; u++) if (b->term_ords[(size_t)q * nt + u] != SB200_NO_TERM) SB_FAIL(SB200_EINVAL, "query %u: SB200_NO_TERM pads the end of a row only", q);
+        for (uint32_t u = t; u < nt; u++) if (ords_in[(size_t)q * nt + u] != SB200_NO_TERM) SB_FAIL(SB200_EINVAL, "query %u: SB200_NO_TERM pads the end of a row only", q);
         break;
       }
       if (ord == SB200_ABSENT_TERM) absent = true;
       else if (ord >= g->n_terms) SB_FAIL(SB200_EINVAL, "query %u: term ordinal %u >= %u", q, ord, g->n_terms);
-      ords[c] = ord; offs[c] = b->offsets ? b->offsets[(size_t)q * nt + t] : t; c++;
+      ords[c] = ord; offs[c] = offsets ? offsets[(size_t)q * nt + t] : t; c++;
     }
     if (c < 2) SB_FAIL(SB200_EINVAL, "query %u has %u terms: a phrase has 2..%d", q, c, MAXT);
-    slop[q] = b->slop ? b->slop[q] : 0u;
-    weight[q] = b->scoring ? b->weights[q] : 0.0f;
+    slop[q] = slops ? slops[q] : 0u;
     if (absent) continue;
     uint32_t max_off = 0, idx[MAXT];
     for (uint32_t i = 0; i < c; i++) { max_off = std::max(max_off, offs[i]); idx[i] = i; }
@@ -824,26 +891,32 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
     for (uint32_t i = 0; i < c; i++) { terms[(size_t)q * nt + i] = ords[idx[i]]; shift[(size_t)q * nt + i] = max_off - offs[idx[i]]; }
     nterms[q] = c;
   }
+  return SB200_OK;
+}
+
+// Candidates (k_phrase_cand<2>) and verification (k_phrase_verify) of planned phrase rows, in groups whose candidate records
+// fit a memory budget; scoring == 0 is exists mode.  After a group's verification the matches of row q are at a3_off[q],
+// ph_mcnt[q] of them (ph_mkey / ph_mdoc, unordered), and done(g0, g1) consumes rows [g0, g1).  kms accumulates the launches.
+typedef std::function<int(uint32_t, uint32_t)> PhraseDone;
+static int phrase_match(sb200_segment* g, uint32_t nq, uint32_t nt, const std::vector<uint32_t>& terms, const std::vector<uint32_t>& shift,
+                        const std::vector<uint32_t>& nterms, const std::vector<uint32_t>& slop, const std::vector<float>& weight, int scoring,
+                        const float* tf_cache256, float& kms, PhraseDone done) {
+  cudaStream_t s = g->stream;
   SB_TRY(ensure(g->q_terms, (size_t)nq * nt)); SB_TRY(ensure(g->ph_shift, (size_t)nq * nt)); SB_TRY(ensure(g->q_nterms, nq));
   SB_TRY(ensure(g->ph_slop, nq)); SB_TRY(ensure(g->ph_weight, nq)); SB_TRY(ensure(g->q_weights, (size_t)nq * nt)); SB_TRY(ensure(g->q_cache, 256));
-  SB_TRY(ensure(g->o_docs, (size_t)nq * k)); SB_TRY(ensure(g->o_scores, (size_t)nq * k)); SB_TRY(ensure(g->o_n, nq));
   SB_TRY(ensure(g->counters, 8)); SB_TRY(ensure(g->a3_off, nq)); SB_TRY(ensure(g->a3_cnt, nq)); SB_TRY(ensure(g->ph_mcnt, nq));
   SB_TRY(ensure(g->ph_ovc, 4)); SB_TRY(ensure(g->ph_pre, (size_t)nq + 1));
-  SB_CUDA(cudaEventRecord(g->ev0, s));
   SB_CUDA(cudaMemcpyAsync(g->q_terms.p, terms.data(), terms.size() * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->ph_shift.p, shift.data(), shift.size() * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->q_nterms.p, nterms.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->ph_slop.p, slop.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemcpyAsync(g->ph_weight.p, weight.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s));
   SB_CUDA(cudaMemsetAsync(g->q_weights.p, 0, (size_t)nq * nt * 4, s));
-  if (b->scoring) SB_CUDA(cudaMemcpyAsync(g->q_cache.p, b->tf_cache256, 256 * 4, cudaMemcpyDefault, s));
+  if (scoring) SB_CUDA(cudaMemcpyAsync(g->q_cache.p, tf_cache256, 256 * 4, cudaMemcpyDefault, s));
   else SB_CUDA(cudaMemsetAsync(g->q_cache.p, 0, 256 * 4, s));
   SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 8 * sizeof(unsigned long long), s));
   SB_CUDA(cudaMemsetAsync(g->a3_cnt.p, 0, (size_t)nq * 4, s));
   SB_CUDA(cudaMemsetAsync(g->ph_mcnt.p, 0, (size_t)nq * 4, s));
-  static size_t sel_conf = 0;
-  const size_t sel_smem = (size_t)A3_SEL_CAP * 8;
-  if (sel_conf < sel_smem) { SB_CUDA(cudaFuncSetAttribute(k_and3_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem)); sel_conf = sel_smem; }
   const size_t cand_smem = (size_t)A3_WARPS * nt * 128 * 12;
   static size_t cand_conf = 0;
   if (cand_conf < cand_smem) { SB_CUDA(cudaFuncSetAttribute(k_phrase_cand<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand_smem)); cand_conf = cand_smem; }
@@ -856,8 +929,6 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
   std::vector<uint64_t> off(nq, 0), pre(nq + 1, 0);
   std::vector<uint32_t> cnt(nq, 0);
   std::vector<AUnit> units;
-  // kernel_ms: the device time of the launches alone (the count read-backs between passes are left out)
-  float kms = 0.0f;
   auto timed = [&](auto&& launch) -> int {
     SB_CUDA(cudaEventRecord(g->evk0, s));
     SB_TRY(launch());
@@ -909,7 +980,7 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
       pos_view(g, V.V);
       V.fieldnorm = g->fieldnorm.p; V.cache = g->q_cache.p;
       V.q_terms = g->q_terms.p; V.q_shift = g->ph_shift.p; V.q_nterms = g->q_nterms.p; V.q_slop = g->ph_slop.p; V.q_weight = g->ph_weight.p;
-      V.nt = nt; V.scoring = b->scoring ? 1 : 0;
+      V.nt = nt; V.scoring = scoring ? 1 : 0;
       V.cand_off = g->a3_off.p; V.cand_pre = g->ph_pre.p; V.slot0 = g0; V.n_slots = ns;
       V.c_doc = g->ph_cdoc.p; V.c_off = g->ph_coff.p; V.c_tf = g->ph_ctf.p;
       V.m_cnt = g->ph_mcnt.p; V.m_key = g->ph_mkey.p; V.m_doc = g->ph_mdoc.p; V.counters = g->counters.p;
@@ -936,12 +1007,44 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
         SB_TRY(timed([&]() -> int { SB_LAUNCH(k_phrase_verify, grid2, PH_WARPS * 32, 0, s, V); SB_CHECK_LAUNCH(); return SB200_OK; }));
       }
     }
-    SB_TRY(timed([&]() -> int {
-      SB_LAUNCH(k_and3_select, ns, 256, sel_smem, s, g->a3_off.p, g->ph_mcnt.p, g->ph_mkey.p, g->ph_mdoc.p, (const uint32_t*)nullptr, g0, k,
-                g->o_docs.p, g->o_scores.p, g->o_n.p);
-      SB_CHECK_LAUNCH(); return SB200_OK; }));
+    SB_TRY(done(g0, g1));
     g0 = g1;
   }
+  return SB200_OK;
+}
+
+// Phrase batch (bm25_phrase.cuh): phrase_rows, phrase_match, then k_and3_select takes every group's top k.
+static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* docs, float* scores, uint32_t* n_out, sb200_phrase_stats* stats) {
+  NvtxRange nvtx("sb200 phrase top-k batch");
+  cudaStream_t s = g->stream;
+  if (!b || !b->term_ords || !docs || !scores || !n_out) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (b->scoring && (!b->weights || !b->tf_cache256)) SB_FAIL(SB200_EINVAL, "scoring needs weights and tf_cache256");
+  if (g->record != SB200_RECORD_FREQS_POSITIONS) SB_FAIL(SB200_EINVAL, "phrase query on a field without positions (record option %d)", g->record);
+  if (!g->has_pos) SB_FAIL(SB200_EINVAL, "phrase query: no positions attached to the segment (sb200_segment_attach_positions)");
+  const uint32_t nq = b->n_queries, nt = b->n_terms, k = b->k;
+  if (nt < 2 || nt > MAXT) SB_FAIL(SB200_ERANGE, "n_terms %u outside [2,%d]", nt, MAXT);
+  if (k == 0 || k > SB200_MAX_K) SB_FAIL(SB200_ERANGE, "k %u outside [1,%d]", k, SB200_MAX_K);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (nq == 0) return SB200_OK;
+  std::vector<uint32_t> terms, shift, nterms, slop;
+  SB_TRY(phrase_rows(g, nq, nt, b->term_ords, b->offsets, b->slop, terms, shift, nterms, slop));
+  std::vector<float> weight(nq, 0.0f);
+  for (uint32_t q = 0; q < nq; q++) weight[q] = b->scoring ? b->weights[q] : 0.0f;
+  SB_TRY(ensure(g->o_docs, (size_t)nq * k)); SB_TRY(ensure(g->o_scores, (size_t)nq * k)); SB_TRY(ensure(g->o_n, nq));
+  SB_CUDA(cudaEventRecord(g->ev0, s));
+  static size_t sel_conf = 0;
+  const size_t sel_smem = (size_t)A3_SEL_CAP * 8;
+  if (sel_conf < sel_smem) { SB_CUDA(cudaFuncSetAttribute(k_and3_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem)); sel_conf = sel_smem; }
+  float kms = 0.0f;
+  SB_TRY(phrase_match(g, nq, nt, terms, shift, nterms, slop, weight, b->scoring, b->tf_cache256, kms, [&](uint32_t g0, uint32_t g1) -> int {
+    SB_CUDA(cudaEventRecord(g->evk0, s));
+    SB_LAUNCH(k_and3_select, g1 - g0, 256, sel_smem, s, g->a3_off.p, g->ph_mcnt.p, g->ph_mkey.p, g->ph_mdoc.p, (const uint32_t*)nullptr, g0, k,
+              g->o_docs.p, g->o_scores.p, g->o_n.p);
+    SB_CHECK_LAUNCH();
+    SB_CUDA(cudaEventRecord(g->evk1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+    return SB200_OK; }));
   SB_TRY(copy_out_tables(g, nq, k, docs, scores, nullptr, n_out));
   unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
@@ -952,6 +1055,262 @@ static int run_phrase(sb200_segment* g, const sb200_phrase_batch* b, uint32_t* d
   if (stats) {
     stats->candidates = h[0]; stats->matches = h[1]; stats->positions_decoded = h[3]; stats->position_bytes = h[4];
     cudaEventElapsedTime(&stats->ms, g->ev0, g->ev1); stats->kernel_ms = kms;
+  }
+  return SB200_OK;
+}
+
+
+// Plan docset stage (bm25_plan.cuh).  The host validates every program, picks each query's cover (BooleanWeight's docset is a
+// subset of it) and splits the batch into groups whose cover fits a memory budget; per group the device decodes the cover,
+// sorts it, runs the programs on it and compacts the survivors, and `emit` receives them: keys (query in group << 32 | doc),
+// ascending, and q_beg, each query's range in them (device and host copies).
+static int run_plan(const sb200_recall_plan_batch* pb, PlanEmit emit, sb200_plan_stats* stats) {
+  NvtxRange nvtx("sb200 recall plan docsets");
+  if (!pb || !pb->segments || pb->n_segments == 0 || !pb->node_off) SB_FAIL(SB200_EINVAL, "NULL argument");
+  const uint32_t nq = pb->n_queries, NS = pb->n_segments;
+  sb200_segment* g = pb->segments[0];
+  if (!g) SB_FAIL(SB200_EINVAL, "plan segment 0 is NULL");
+  for (uint32_t i = 0; i < NS; i++) {
+    const sb200_segment* x = pb->segments[i];
+    if (!x || x->device != g->device || x->max_doc != g->max_doc) SB_FAIL(SB200_EINVAL, "plan segment %u: NULL, or another max_doc / device than segment 0", i);
+  }
+  if (nq && pb->node_off[nq] > pb->node_off[0] && !pb->nodes) SB_FAIL(SB200_EINVAL, "NULL nodes");
+  const auto t0 = std::chrono::steady_clock::now();
+  SB_CUDA(cudaSetDevice(g->device));
+  cudaStream_t s = g->stream;
+  // ---- phrase leaves: every distinct (segment, row) is planned once (phrase_rows); its matching documents come later
+  const uint32_t PT = pb->phrase_terms;
+  std::vector<std::vector<uint32_t>> seg_rows(NS);          // per segment: the phrase rows its PHRASE nodes use
+  std::vector<uint32_t> ph_index;                           // per node of the batch: the distinct phrase of a PHRASE node
+  std::vector<uint64_t> ph_key;                             // per distinct phrase: segment << 32 | row
+  {
+    const uint32_t nn = nq ? pb->node_off[nq] : 0u;
+    ph_index.assign(nn, 0);
+    for (uint32_t x = 0; x < nn; x++) {
+      const sb200_plan_node& N = pb->nodes[x];
+      if (N.kind != SB200_PLAN_PHRASE) continue;
+      if (N.segment >= NS) SB_FAIL(SB200_EINVAL, "node %u: segment %u >= %u", x, N.segment, NS);
+      if (N.arg >= pb->n_phrases || !pb->phrase_ords) SB_FAIL(SB200_EINVAL, "node %u: phrase row %u >= %u", x, N.arg, pb->n_phrases);
+      const sb200_segment* sg = pb->segments[N.segment];
+      if (sg->record != SB200_RECORD_FREQS_POSITIONS || !sg->has_pos) SB_FAIL(SB200_EINVAL, "node %u: phrase leaf on plan segment %u, which has no positions", x, N.segment);
+      ph_key.push_back(((uint64_t)N.segment << 32) | N.arg);
+    }
+    std::sort(ph_key.begin(), ph_key.end()); ph_key.erase(std::unique(ph_key.begin(), ph_key.end()), ph_key.end());
+    for (uint32_t x = 0; x < nn; x++) if (pb->nodes[x].kind == SB200_PLAN_PHRASE)
+      ph_index[x] = (uint32_t)(std::lower_bound(ph_key.begin(), ph_key.end(), ((uint64_t)pb->nodes[x].segment << 32) | pb->nodes[x].arg) - ph_key.begin());
+    if (!ph_key.empty() && (PT < 2 || PT > (uint32_t)MAXT)) SB_FAIL(SB200_ERANGE, "phrase_terms %u outside [2,%d]", PT, MAXT);
+    for (uint64_t kk : ph_key) seg_rows[kk >> 32].push_back((uint32_t)kk);
+  }
+  // per segment with phrases: the planned rows (terms in Intersection order; nterms 0 = a term is absent, the phrase is empty)
+  std::vector<std::vector<uint32_t>> pr_terms(NS), pr_shift(NS), pr_nterms(NS), pr_slop(NS);
+  for (uint32_t si = 0; si < NS; si++) {
+    const std::vector<uint32_t>& rows = seg_rows[si];
+    if (rows.empty()) continue;
+    std::vector<uint32_t> ords(rows.size() * PT), offs(rows.size() * PT), sl(rows.size());
+    for (size_t i = 0; i < rows.size(); i++) {
+      for (uint32_t t = 0; t < PT; t++) {
+        ords[i * PT + t] = pb->phrase_ords[(size_t)rows[i] * PT + t];
+        offs[i * PT + t] = pb->phrase_offsets ? pb->phrase_offsets[(size_t)rows[i] * PT + t] : t;
+      }
+      sl[i] = pb->phrase_slop ? pb->phrase_slop[rows[i]] : 0u;
+    }
+    SB_TRY(phrase_rows(pb->segments[si], (uint32_t)rows.size(), PT, ords.data(), offs.data(), sl.data(), pr_terms[si], pr_shift[si], pr_nterms[si], pr_slop[si]));
+  }
+  auto ph_plan = [&](uint32_t i, uint32_t& si, uint32_t& r) {   // distinct phrase -> (segment, index among its rows)
+    si = (uint32_t)(ph_key[i] >> 32);
+    r = (uint32_t)(std::lower_bound(seg_rows[si].begin(), seg_rows[si].end(), (uint32_t)ph_key[i]) - seg_rows[si].begin());
+  };
+  // ---- programs and covers
+  struct Cov { uint64_t cost = 0; std::vector<uint64_t> leaves; };   // leaves: segment << 32 | ordinal
+  std::vector<std::vector<uint64_t>> cover(nq);
+  std::vector<uint64_t> cost(nq, 0);
+  for (uint32_t q = 0; q < nq; q++) {
+    const uint32_t n0 = pb->node_off[q], n1 = pb->node_off[q + 1];
+    if (n1 < n0 || n1 - n0 == 0 || n1 - n0 > SB200_PLAN_MAX_NODES) SB_FAIL(SB200_EINVAL, "query %u: %d nodes (1..%d)", q, (int)(n1 - n0), SB200_PLAN_MAX_NODES);
+    std::vector<Cov> st;
+    std::vector<uint8_t> occ;
+    for (uint32_t x = n0; x < n1; x++) {
+      const sb200_plan_node& N = pb->nodes[x];
+      if (N.occur > SB200_PLAN_MUST_NOT) SB_FAIL(SB200_EINVAL, "query %u node %u: occur %u", q, x - n0, (unsigned)N.occur);
+      Cov c;
+      if (N.kind == SB200_PLAN_TERM) {
+        if (N.segment >= NS) SB_FAIL(SB200_EINVAL, "query %u node %u: segment %u >= %u", q, x - n0, N.segment, NS);
+        if (N.arg != SB200_ABSENT_TERM) {
+          const sb200_segment* sg = pb->segments[N.segment];
+          if (N.arg >= sg->n_terms) SB_FAIL(SB200_EINVAL, "query %u node %u: term ordinal %u >= %u", q, x - n0, N.arg, sg->n_terms);
+          c.cost = sg->h_df[N.arg]; c.leaves.push_back(((uint64_t)N.segment << 32) | N.arg);
+        }
+      } else if (N.kind == SB200_PLAN_PHRASE) {   // cover: the postings of the phrase's rarest term
+        uint32_t si, r;
+        ph_plan(ph_index[x], si, r);
+        if (pr_nterms[si][r]) {
+          const uint32_t ord = pr_terms[si][(size_t)r * PT];
+          c.cost = pb->segments[si]->h_df[ord]; c.leaves.push_back(((uint64_t)si << 32) | ord);
+        }
+      } else if (N.kind == SB200_PLAN_BOOL) {
+        const uint32_t nc = N.n_children;
+        if (nc > st.size()) SB_FAIL(SB200_EINVAL, "query %u node %u: %u children, %zu values on the stack", q, x - n0, nc, st.size());
+        const size_t b = st.size() - nc;
+        bool has_must = false;
+        for (size_t i = b; i < st.size(); i++) has_must |= occ[i] == SB200_PLAN_MUST;
+        if (nc == 1 && occ[b] != SB200_PLAN_MUST_NOT) c = st[b];
+        else if (nc > 1 && has_must) {   // the cheapest Must clause
+          size_t best = SIZE_MAX;
+          for (size_t i = b; i < st.size(); i++) if (occ[i] == SB200_PLAN_MUST && (best == SIZE_MAX || st[i].cost < st[best].cost)) best = i;
+          c = st[best];
+        } else if (nc > 1) {             // the union of the Should clauses
+          for (size_t i = b; i < st.size(); i++) if (occ[i] == SB200_PLAN_SHOULD) { c.cost += st[i].cost; c.leaves.insert(c.leaves.end(), st[i].leaves.begin(), st[i].leaves.end()); }
+        }
+        st.resize(b); occ.resize(b);
+      } else if (N.kind != SB200_PLAN_EMPTY) {
+        SB_FAIL(SB200_EINVAL, "query %u node %u: kind %u", q, x - n0, (unsigned)N.kind);
+      }
+      st.push_back(std::move(c)); occ.push_back(N.occur);
+    }
+    if (st.size() != 1) SB_FAIL(SB200_EINVAL, "query %u: the program leaves %zu values (1 expected)", q, st.size());
+    std::vector<uint64_t>& L = st[0].leaves;
+    std::sort(L.begin(), L.end()); L.erase(std::unique(L.begin(), L.end()), L.end());
+    for (uint64_t l : L) cost[q] += pb->segments[l >> 32]->h_df[(uint32_t)l];
+    cover[q] = std::move(L);
+  }
+  // ---- the matching documents of every distinct phrase (exists mode), ascending, concatenated in ph_key order
+  float kms = 0.0f;
+  std::vector<uint32_t> ph_off(ph_key.size() + 1, 0), ph_docs;
+  {
+    std::vector<std::vector<uint32_t>> lists(ph_key.size());
+    for (uint32_t si = 0; si < NS; si++) {
+      const uint32_t nr = (uint32_t)seg_rows[si].size();
+      if (!nr) continue;
+      sb200_segment* sg = pb->segments[si];
+      const uint32_t base = (uint32_t)(std::lower_bound(ph_key.begin(), ph_key.end(), (uint64_t)si << 32) - ph_key.begin());
+      std::vector<float> w(nr, 0.0f);
+      std::vector<uint32_t> mc; std::vector<uint64_t> mo;
+      SB_TRY(phrase_match(sg, nr, PT, pr_terms[si], pr_shift[si], pr_nterms[si], pr_slop[si], w, 0, nullptr, kms, [&](uint32_t a0, uint32_t a1) -> int {
+        mc.resize(a1 - a0); mo.resize(a1 - a0);
+        SB_CUDA(cudaMemcpyAsync(mc.data(), sg->ph_mcnt.p + a0, (size_t)(a1 - a0) * 4, cudaMemcpyDeviceToHost, sg->stream));
+        SB_CUDA(cudaMemcpyAsync(mo.data(), sg->a3_off.p + a0, (size_t)(a1 - a0) * 8, cudaMemcpyDeviceToHost, sg->stream));
+        SB_CUDA(cudaStreamSynchronize(sg->stream));
+        for (uint32_t i = 0; i < a1 - a0; i++) {
+          std::vector<uint32_t>& L = lists[base + a0 + i];
+          L.resize(mc[i]);
+          if (mc[i]) SB_CUDA(cudaMemcpy(L.data(), sg->ph_mdoc.p + mo[i], (size_t)mc[i] * 4, cudaMemcpyDeviceToHost));
+          std::sort(L.begin(), L.end());
+        }
+        return SB200_OK; }));
+      unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      SB_CUDA(cudaMemcpyAsync(h, sg->counters.p, sizeof(h), cudaMemcpyDeviceToHost, sg->stream));
+      SB_CUDA(cudaStreamSynchronize(sg->stream));
+      if (h[2]) SB_FAIL(SB200_EFORMAT, "%llu phrase work items met inconsistent posting / position data", h[2]);
+      if (h[5]) SB_FAIL(SB200_ENOMEM, "phrase verification: %llu candidates need carrying-slop buffers beyond 2^32 entries", h[5]);
+    }
+    for (size_t i = 0; i < lists.size(); i++) {
+      if ((uint64_t)ph_docs.size() + lists[i].size() > 0xFFFFFFFFull) SB_FAIL(SB200_ERANGE, "phrase leaves match more than 2^32 documents in all");
+      ph_docs.insert(ph_docs.end(), lists[i].begin(), lists[i].end());
+      ph_off[i + 1] = (uint32_t)ph_docs.size();
+    }
+  }
+  std::vector<sb200_plan_node> hn(pb->nodes, pb->nodes + (nq ? pb->node_off[nq] : 0u));   // PHRASE args -> distinct phrase
+  for (size_t x = 0; x < hn.size(); x++) if (hn[x].kind == SB200_PLAN_PHRASE) hn[x].arg = ph_index[x];
+  SB_TRY(ensure(g->pl_ph_off, ph_off.size())); SB_TRY(ensure(g->pl_ph_docs, std::max<size_t>(ph_docs.size(), 1)));
+  SB_CUDA(cudaMemcpyAsync(g->pl_ph_off.p, ph_off.data(), ph_off.size() * 4, cudaMemcpyHostToDevice, s));
+  if (!ph_docs.empty()) SB_CUDA(cudaMemcpyAsync(g->pl_ph_docs.p, ph_docs.data(), ph_docs.size() * 4, cudaMemcpyHostToDevice, s));
+  std::vector<PSeg> hs(NS);
+  for (uint32_t i = 0; i < NS; i++) {
+    memset(&hs[i], 0, sizeof(PSeg));
+    const sb200_segment* x = pb->segments[i];
+    seg_view(x, hs[i].S); hs[i].a128 = x->a_post.p; hs[i].t_aoff = x->t_aoff.p; hs[i].n_terms = x->n_terms;
+  }
+  SB_TRY(ensure(g->pl_segs, NS * sizeof(PSeg))); SB_TRY(ensure(g->counters, 4));
+  SB_CUDA(cudaMemcpyAsync(g->pl_segs.p, hs.data(), NS * sizeof(PSeg), cudaMemcpyHostToDevice, s));
+  SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 4 * sizeof(unsigned long long), s));
+  // candidate keys twice (sort), a flag, the compacted keys: ~32 B per candidate
+  uint64_t budget = (uint64_t)2 << 30;
+  if (const char* e = getenv("SB200_PLAN_BUDGET_MB")) { const long mb = atol(e); if (mb > 0) budget = (uint64_t)mb << 20; }
+  const uint64_t max_entries = std::max<uint64_t>(budget / 32, 1);
+  uint64_t n_cover = 0, n_docs = 0;
+  uint32_t n_groups = 0;
+  auto timed = [&](auto&& launch) -> int {
+    SB_CUDA(cudaEventRecord(g->evk0, s));
+    SB_TRY(launch());
+    SB_CUDA(cudaEventRecord(g->evk1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+    return SB200_OK;
+  };
+  std::vector<PCover> units;
+  std::vector<uint32_t> chunks, noff;
+  std::vector<uint64_t> beg;
+  uint32_t g0 = 0;
+  while (g0 < nq) {
+    uint64_t E = 0; uint32_t g1 = g0;
+    while (g1 < nq && (g1 == g0 || E + cost[g1] <= max_entries)) E += cost[g1++];
+    const uint32_t n = g1 - g0;
+    units.clear(); chunks.clear(); noff.assign(n + 1, 0); beg.assign(n + 1, 0);
+    uint64_t at = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      beg[i] = at;
+      for (uint64_t l : cover[g0 + i]) {
+        const uint32_t sg = (uint32_t)(l >> 32), ord = (uint32_t)l, df = pb->segments[sg]->h_df[ord];
+        const uint32_t nblk = (df >> 7) + ((df & 127u) ? 1u : 0u);
+        for (uint32_t b = 0; b < nblk; b++) { PCover c; c.q = i; c.seg = sg; c.ord = ord; c.blk = b; c.out = at + (uint64_t)b * 128; units.push_back(c); }
+        at += df;
+      }
+      for (uint64_t c = beg[i]; c < at; c += 32) chunks.push_back((uint32_t)c);
+      noff[i + 1] = pb->node_off[g0 + i + 1] - pb->node_off[g0];
+    }
+    beg[n] = at;
+    const size_t ne = std::max<uint64_t>(E, 1), nn = noff[n];
+    SB_TRY(ensure(g->pl_keys, ne)); SB_TRY(ensure(g->pl_keys2, ne)); SB_TRY(ensure(g->pl_keep, ne)); SB_TRY(ensure(g->pl_beg, n + 1));
+    SB_TRY(ensure(g->pl_cover, std::max<size_t>(units.size(), 1) * sizeof(PCover))); SB_TRY(ensure(g->pl_units, std::max<size_t>(chunks.size(), 1)));
+    SB_TRY(ensure(g->pl_nodes, nn * sizeof(sb200_plan_node))); SB_TRY(ensure(g->pl_off, n + 1)); SB_TRY(ensure(g->pl_cnt, 1));
+    SB_CUDA(cudaMemcpyAsync(g->pl_nodes.p, hn.data() + pb->node_off[g0] - pb->node_off[0], nn * sizeof(sb200_plan_node), cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->pl_off.p, noff.data(), (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->pl_beg.p, beg.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (!units.empty()) SB_CUDA(cudaMemcpyAsync(g->pl_cover.p, units.data(), units.size() * sizeof(PCover), cudaMemcpyHostToDevice, s));
+    if (!chunks.empty()) SB_CUDA(cudaMemcpyAsync(g->pl_units.p, chunks.data(), chunks.size() * 4, cudaMemcpyHostToDevice, s));
+    PlanParams P;
+    memset(&P, 0, sizeof(P));
+    P.segs = (const PSeg*)g->pl_segs.p; P.nodes = (const sb200_plan_node*)g->pl_nodes.p; P.node_off = g->pl_off.p;
+    P.cover = (const PCover*)g->pl_cover.p; P.n_cover = (uint32_t)units.size();
+    P.ph_off = g->pl_ph_off.p; P.ph_docs = g->pl_ph_docs.p;
+    P.q_beg = g->pl_beg.p; P.units = g->pl_units.p; P.n_units = (uint32_t)chunks.size(); P.keep = g->pl_keep.p; P.counters = g->counters.p;
+    uint64_t n_keep = 0;
+    if (E) {
+      P.keys = g->pl_keys.p; P.n_keys = E;
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_plan_cover, div_up(units.size(), PL_WARPS), PL_WARPS * 32, 0, s, P); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      int qbits = 1; while ((1u << qbits) < n) qbits++;
+      cub::DoubleBuffer<uint64_t> dk(g->pl_keys.p, g->pl_keys2.p);
+      size_t need = 0;
+      SB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, need, dk, (int64_t)E, 0, 32 + qbits, s));
+      SB_TRY(ensure(g->pl_tmp, need + 256));
+      SB_TRY(timed([&]() -> int { SB_CUDA(cub::DeviceRadixSort::SortKeys(g->pl_tmp.p, need, dk, (int64_t)E, 0, 32 + qbits, s)); return SB200_OK; }));
+      P.keys = dk.Current();
+      uint64_t* out = dk.Alternate();
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_plan_eval, div_up(chunks.size(), PL_WARPS), PL_WARPS * 32, 0, s, P); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      need = 0;
+      SB_CUDA(cub::DeviceSelect::Flagged(nullptr, need, dk.Current(), g->pl_keep.p, out, g->pl_cnt.p, (int64_t)E, s));
+      SB_TRY(ensure(g->pl_tmp, need + 256));
+      SB_TRY(timed([&]() -> int { SB_CUDA(cub::DeviceSelect::Flagged(g->pl_tmp.p, need, dk.Current(), g->pl_keep.p, out, g->pl_cnt.p, (int64_t)E, s)); return SB200_OK; }));
+      SB_CUDA(cudaMemcpyAsync(&n_keep, g->pl_cnt.p, 8, cudaMemcpyDeviceToHost, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_plan_bounds, div_up(n + 1, 256), 256, 0, s, out, n_keep, n, g->pl_beg.p); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      SB_CUDA(cudaMemcpyAsync(beg.data(), g->pl_beg.p, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s));
+      unsigned long long h[4] = {0, 0, 0, 0};
+      SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      if (h[2]) SB_FAIL(SB200_EFORMAT, "%llu plan work items met inconsistent posting data", h[2]);
+      P.keys = out;
+    } else {
+      P.keys = g->pl_keys.p;
+    }
+    n_cover += E; n_docs += n_keep; n_groups++;
+    SB_CUDA(cudaStreamSynchronize(s));   // emit may work on another stream: every upload and launch of the group is complete
+    SB_TRY(emit(g0, g1, P.keys, g->pl_beg.p, beg));
+    g0 = g1;
+  }
+  if (stats) {
+    stats->cover = n_cover; stats->docs = n_docs; stats->groups = n_groups; stats->_pad = 0;
+    stats->ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); stats->kernel_ms = kms;
   }
   return SB200_OK;
 }
@@ -1763,6 +2122,38 @@ void sb200_docset_destroy(sb200_docset* ds) {
   if (!ds) return;
   cudaSetDevice(ds->device);
   delete ds;
+}
+
+int sb200_recall_plan_docs(const sb200_recall_plan_batch* plan, uint64_t* counts, uint32_t* docs, uint64_t cap, sb200_plan_stats* stats) {
+  if (!plan || !counts || (cap && !docs)) SB_FAIL(SB200_EINVAL, "NULL argument");
+  std::vector<uint32_t> h;
+  auto emit = [&](uint32_t g0, uint32_t g1, const uint64_t* keys, const uint64_t*, const std::vector<uint64_t>& beg) -> int {
+    const uint32_t n = g1 - g0;
+    std::vector<uint64_t> c(n);
+    for (uint32_t i = 0; i < n; i++) c[i] = beg[i + 1] - beg[i];
+    SB_CUDA(cudaMemcpy(counts + g0, c.data(), (size_t)n * 8, cudaMemcpyDefault));
+    if (!cap || beg[n] == 0) return SB200_OK;
+    sb200_segment* g = plan->segments[0];
+    DevBuf<uint32_t> d;
+    SB_TRY(d.alloc(beg[n]));
+    SB_LAUNCH(k_plan_docs, div_up(beg[n], 256), 256, 0, g->stream, keys, beg[n], d.p);
+    SB_CHECK_LAUNCH();
+    h.resize(beg[n]);
+    SB_CUDA(cudaMemcpyAsync(h.data(), d.p, beg[n] * 4, cudaMemcpyDeviceToHost, g->stream));
+    SB_CUDA(cudaStreamSynchronize(g->stream));
+    for (uint32_t i = 0; i < n; i++) {
+      const uint64_t c = std::min<uint64_t>(cap, beg[i + 1] - beg[i]);
+      if (c) SB_CUDA(cudaMemcpy(docs + (size_t)(g0 + i) * cap, h.data() + beg[i], c * 4, cudaMemcpyDefault));
+    }
+    return SB200_OK;
+  };
+  return run_plan(plan, emit, stats);
+}
+
+int sb200_multi_signal_topk_batch_plan(const sb200_multi_signal_batch* batch, const sb200_recall_plan_batch* plan, const sb200_optic_batch* optic,
+                                       uint32_t* docs, double* totals, uint32_t* n_out, sb200_bm25_stats* stats) {
+  if (!plan) SB_FAIL(SB200_EINVAL, "NULL plan batch");
+  return run_multi(batch, optic, docs, totals, n_out, stats, plan);
 }
 
 int sb200_multi_signal_topk_batch_optic(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, uint32_t* docs,

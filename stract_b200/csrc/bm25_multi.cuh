@@ -61,6 +61,98 @@ __host__ __device__ constexpr size_t m_warp_smem() { return (size_t)TMAX * 128 *
 template <int TMAX>
 __host__ __device__ constexpr size_t m_cta_smem() { return M_MAX_FIELDS * 256 * 4 + M_MAX_OPS * sizeof(MOp) + WQ * m_warp_smem<TMAX>(); }
 
+// The per-candidate signal program of one document with the term frequencies of its T slots known (tf 0 = the slot does not
+// hold it): the ops in order, the rule-slot boosts, then (OPTIC) the docset-rule boosts.  k_sig_multi and k_plan_recall
+// (bm25_plan.cuh) both call it, so a document gets the same f64 total whichever kernel found it.
+template <int TMAX, bool OPTIC>
+__device__ __forceinline__ double m_total(const MParams& P, const MOp* s_ops, const float* s_cache, const uint32_t* s_nf, const uint32_t* s_fld,
+                                          const float* s_wf, const OTerm* tc, uint32_t T, uint32_t q, uint32_t d, const uint32_t (&tf)[TMAX],
+                                          uint32_t o_q, uint32_t o_nr) {
+  const uint32_t SM = P.n_slots_max;
+  const double DAMP[3] = {1.0, 0.4, 0.4 * 0.4};   // NGRAM_DAMPENING.powi(hits) (order.rs:99,127)
+  uint32_t fid[M_MAX_FIELDS];
+#pragma unroll
+  for (int f = 0; f < M_MAX_FIELDS; f++) fid[f] = ((uint32_t)f < P.n_fields) ? P.fields[f].S.fieldnorm[d] : 0u;
+  double total = 0.0;
+  int hits = 0;
+  for (uint32_t o = 0; o < P.n_ops; o++) {
+    const MOp op = s_ops[o];
+    double sc = 0.0;
+    if (op.kind == 4u) {
+      sc = P.sig[(size_t)d * P.n_cols + op.col];
+    } else if (op.kind == 1u) {
+      // Bm25F: text_fields.values_mut().map(|f| f.bm25f(doc)).sum::<f64>() -- fields in EnumMap order, a field
+      // without query terms is not in the map
+#pragma unroll
+      for (int f = 0; f < M_MAX_FIELDS; f++) {
+        if ((uint32_t)f >= P.n_fields || s_nf[f] == 0) continue;
+        const float norm = s_cache[f * 256 + fid[f]], k1p1 = P.fields[f].k1p1, coef = P.fields[f].coef;
+        float b = 0.0f;
+#pragma unroll
+        for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == (uint32_t)f) {
+          float part = 0.0f;
+          if (tf[x]) { const float t = __fmul_rn((float)tf[x], coef); part = __fmul_rn(s_wf[x], __fdiv_rn(__fmul_rn(t, k1p1), __fadd_rn(t, norm))); }
+          b = __fadd_rn(b, part);
+        }
+        sc = __dadd_rn(sc, (double)b);
+      }
+    } else if (s_nf[op.field] != 0) {
+      const uint32_t f = op.field;
+      if (op.kind == 0u) {
+        const float norm = s_cache[f * 256 + fid[f]], k1p1 = P.fields[f].k1p1;
+        float b = 0.0f;
+#pragma unroll
+        for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f) {
+          float part = 0.0f;
+          if (tf[x]) { const float t = (float)tf[x]; part = __fmul_rn(tc[x].weight, __fdiv_rn(__fmul_rn(t, k1p1), __fadd_rn(t, norm))); }
+          b = __fadd_rn(b, part);
+        }
+        sc = (double)b;
+      } else if (op.kind == 2u) {
+        double n = 0.0;
+#pragma unroll
+        for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f) n = __dadd_rn(n, tf[x] ? 1.0 : 0.0);
+        sc = __ddiv_rn(n, (double)s_nf[f]);
+      } else if (op.kind == 3u) {
+        float b = 0.0f;
+#pragma unroll
+        for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f && tf[x]) b = __fadd_rn(b, tc[x].weight);
+        sc = (double)b;
+      }
+    }
+    if (op.chain) {
+      if (op.chain == 1u) hits = 0;
+      sc = __dmul_rn(sc, DAMP[hits > 2 ? 2 : hits]);
+      if (sc > 0.0) hits++;
+    }
+    total = __dadd_rn(total, __dmul_rn(op.coeff, sc));
+  }
+  if (P.q_boost) {   // SignalComputer::boosts
+    double down = 0.0, up = 0.0;
+#pragma unroll
+    for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && (s_fld[x] & 0x80u) && tf[x]) {
+      const double b = P.q_boost[(size_t)q * SM + x];
+      if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
+    }
+    const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
+    total = __dmul_rn(total, factor);
+  }
+  if constexpr (OPTIC) {
+    if (o_nr) {   // SignalComputer::boosts over the rule docsets, in rule order
+      double down = 0.0, up = 0.0;
+      for (uint32_t r = 0; r < o_nr; r++) {
+        const size_t at = (size_t)o_q * P.d_max_rules + r;
+        if (!m_in(P.d_bits[P.d_rule[at]], d)) continue;
+        const double b = P.d_boost[at];
+        if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
+      }
+      const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
+      total = __dmul_rn(total, factor);
+    }
+  }
+  return total;
+}
+
 template <int TMAX, bool OPTIC = false>
 __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
   SB_DYN_SMEM(smem_raw);
@@ -140,7 +232,6 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
   bool thr_on = false; uint64_t thr_hi = 0; uint32_t thr_lo = 0;   // warp-uniform
   unsigned long long my_docs = 0, my_blocks = 0;
   bool watchdog = false, bad_doc = false;
-  const double DAMP[3] = {1.0, 0.4, 0.4 * 0.4};   // NGRAM_DAMPENING.powi(hits) (order.rs:99,127)
 
   while (T > 0) {
     if (budget-- == 0) { watchdog = true; break; }
@@ -232,86 +323,7 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
         if (o_rq && !m_in(o_rq, d)) continue;   // DiscardNonMatching
       }
       my_docs++;
-      uint32_t fid[M_MAX_FIELDS];
-#pragma unroll
-      for (int f = 0; f < M_MAX_FIELDS; f++) fid[f] = ((uint32_t)f < P.n_fields) ? P.fields[f].S.fieldnorm[d] : 0u;
-      double total = 0.0;
-      int hits = 0;
-      for (uint32_t o = 0; o < P.n_ops; o++) {
-        const MOp op = s_ops[o];
-        double sc = 0.0;
-        if (op.kind == 4u) {
-          sc = P.sig[(size_t)d * P.n_cols + op.col];
-        } else if (op.kind == 1u) {
-          // Bm25F: text_fields.values_mut().map(|f| f.bm25f(doc)).sum::<f64>() -- fields in EnumMap order, a field
-          // without query terms is not in the map
-#pragma unroll
-          for (int f = 0; f < M_MAX_FIELDS; f++) {
-            if ((uint32_t)f >= P.n_fields || s_nf[f] == 0) continue;
-            const float norm = s_cache[f * 256 + fid[f]], k1p1 = P.fields[f].k1p1, coef = P.fields[f].coef;
-            float b = 0.0f;
-#pragma unroll
-            for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == (uint32_t)f) {
-              float part = 0.0f;
-              if (tf[x]) { const float t = __fmul_rn((float)tf[x], coef); part = __fmul_rn(s_wf[x], __fdiv_rn(__fmul_rn(t, k1p1), __fadd_rn(t, norm))); }
-              b = __fadd_rn(b, part);
-            }
-            sc = __dadd_rn(sc, (double)b);
-          }
-        } else if (s_nf[op.field] != 0) {
-          const uint32_t f = op.field;
-          if (op.kind == 0u) {
-            const float norm = s_cache[f * 256 + fid[f]], k1p1 = P.fields[f].k1p1;
-            float b = 0.0f;
-#pragma unroll
-            for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f) {
-              float part = 0.0f;
-              if (tf[x]) { const float t = (float)tf[x]; part = __fmul_rn(tc[x].weight, __fdiv_rn(__fmul_rn(t, k1p1), __fadd_rn(t, norm))); }
-              b = __fadd_rn(b, part);
-            }
-            sc = (double)b;
-          } else if (op.kind == 2u) {
-            double n = 0.0;
-#pragma unroll
-            for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f) n = __dadd_rn(n, tf[x] ? 1.0 : 0.0);
-            sc = __ddiv_rn(n, (double)s_nf[f]);
-          } else if (op.kind == 3u) {
-            float b = 0.0f;
-#pragma unroll
-            for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && s_fld[x] == f && tf[x]) b = __fadd_rn(b, tc[x].weight);
-            sc = (double)b;
-          }
-        }
-        if (op.chain) {
-          if (op.chain == 1u) hits = 0;
-          sc = __dmul_rn(sc, DAMP[hits > 2 ? 2 : hits]);
-          if (sc > 0.0) hits++;
-        }
-        total = __dadd_rn(total, __dmul_rn(op.coeff, sc));
-      }
-      if (P.q_boost) {   // SignalComputer::boosts
-        double down = 0.0, up = 0.0;
-#pragma unroll
-        for (int x = 0; x < TMAX; x++) if ((uint32_t)x < T && (s_fld[x] & 0x80u) && tf[x]) {
-          const double b = P.q_boost[(size_t)q * SM + x];
-          if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
-        }
-        const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
-        total = __dmul_rn(total, factor);
-      }
-      if constexpr (OPTIC) {
-        if (o_nr) {   // SignalComputer::boosts over the rule docsets, in rule order
-          double down = 0.0, up = 0.0;
-          for (uint32_t r = 0; r < o_nr; r++) {
-            const size_t at = (size_t)o_q * P.d_max_rules + r;
-            if (!m_in(P.d_bits[P.d_rule[at]], d)) continue;
-            const double b = P.d_boost[at];
-            if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
-          }
-          const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
-          total = __dmul_rn(total, factor);
-        }
-      }
+      const double total = m_total<TMAX, OPTIC>(P, s_ops, s_cache, s_nf, s_fld, s_wf, tc, T, q, d, tf, o_q, o_nr);
       const uint64_t kh = ord_f64(total);
       const uint32_t kl = ~d;
       if (thr_on && !key_gt(kh, kl, thr_hi, thr_lo)) continue;
