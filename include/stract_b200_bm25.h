@@ -389,6 +389,47 @@ SB200_API int sb200_multi_signal_topk_batch_plan(const sb200_multi_signal_batch*
                                                  const sb200_optic_batch* optic, uint32_t* docs, double* totals, uint32_t* n_out,
                                                  sb200_bm25_stats* stats);
 
+/* ---- the recall webpages of Stract's searcher (retrieve_ranking_websites, core/src/inverted_index/search.rs:110-192) ----------
+ * For a GIVEN list of documents per query, what LocalRecallRankingWebpage::new (core/src/ranking/pipeline/stages/recall.rs:167-220)
+ * takes from the SignalComputer, evaluated with the slots, ops and optic rules of the top-k entry points (same batch, same optic
+ * batch; optic nullable):
+ *   values / scores [n_queries][n_docs_max][n_ops]  op o's SignalCalculation { value, score } (compute_signals, signals/mod.rs:376-388):
+ *       BM25, BM25F, COVERAGE, IDF_SUM: value = the op's score before n-gram dampening, score = after it (computer/order.rs:113-136);
+ *       NUMERIC: score = the signal table's column; value is NOT written -- a numeric CoreSignal's value is its raw fast-field
+ *       value as f64 (signals/core/non_text.rs), which the caller holds.
+ *     sum over o (in op order) of coeff_o * score_o, times boost, is bit for bit the total the top-k entry points give the document.
+ *   boosts [n_queries][n_docs_max]  SignalComputer::boosts (computer/mod.rs:471-497) over the rule slots and the docset rules; 1.0
+ *       without rules.  The optic exclude / require filters are NOT applied: the caller chose the documents.
+ *   min_slop [n_queries][n_docs_max][2]  per distance field (dist_field[0] = Title, [1] = CleanBody) min_slop of term_distance.rs:23-54
+ *       over the field's TEXT slots in slot order (rule slots are not postings of the field; duplicate terms are separate slots),
+ *       positions absolute (positions_with_offset(0)): the max over consecutive slot pairs of the least b - a with a in the left
+ *       list and b > a in the right one.  0xFFFFFFFF (u32::MAX) when the field is not registered, has fewer than 2 slots, or a slot
+ *       lacks the document (an absent term included: SegmentPostings::empty()).  MinTitleSlop / MinCleanBodySlop are then
+ *       { value: v as f64, score: 1.0 / (v as f64 + 1.0) } in f64.
+ * Documents may come in any order and repeat; every output follows the caller's order (search.rs restores orig_index).  docs and
+ * n_docs are host memory; the four outputs host or device memory.  Entries past n_docs[q] are 0 (values: left as they were).
+ * SB200_EINVAL: a doc >= max_doc, n_docs[q] > n_docs_max, a distance field index >= n_fields or both the same, a distance field
+ * whose segment has no positions attached (sb200_segment_attach_positions), rule slots and docset rules in one query; the batch's
+ * limits are those of sb200_multi_signal_topk_batch (k is not read).  Scratch grows with the batch; SB200_ENOMEM when it cannot. */
+#define SB200_WEBPAGE_NO_FIELD 0xFFFFFFFFu
+typedef struct {
+  uint32_t n_queries, n_docs_max;   /* n_queries must equal the signal batch's; n_docs_max = row width of docs */
+  const uint32_t* docs;             /* [n_queries * n_docs_max] */
+  const uint32_t* n_docs;           /* [n_queries] */
+  uint32_t dist_field[2];           /* indices into batch->fields of Title and CleanBody, SB200_WEBPAGE_NO_FIELD when not registered */
+} sb200_webpage_batch;
+typedef struct {
+  double* values;                   /* [n_queries][n_docs_max][n_ops] */
+  double* scores;                   /* [n_queries][n_docs_max][n_ops] */
+  double* boosts;                   /* [n_queries][n_docs_max] */
+  uint32_t* min_slop;               /* [n_queries][n_docs_max][2] */
+} sb200_webpage_out;
+/* docs: documents evaluated; docs_with_positions: documents with at least one distance field decided by its positions;
+ * positions_decoded / position_bytes as sb200_phrase_stats; ms: the whole call, kernel_ms: the launches (CUDA events). */
+typedef struct { uint64_t docs, docs_with_positions, positions_decoded, position_bytes; float ms, kernel_ms; } sb200_webpage_stats;
+SB200_API int sb200_multi_signal_webpages(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic,
+                                          const sb200_webpage_batch* wb, const sb200_webpage_out* out, sb200_webpage_stats* stats);
+
 /* idf(doc_freq, doc_count) = ln(1 + (N - n + 0.5) / (n + 0.5)) in f32 (tantivy/src/query/bm25.rs:52-56,
  * core/src/ranking/bm25.rs:23-27) for an array of doc_freqs; tantivy_weight != 0 returns Bm25Weight.weight = idf * (1 + K1). */
 SB200_API int sb200_bm25_idf(const uint32_t* doc_freq, uint64_t n, uint64_t doc_count, int tantivy_weight, float* out);

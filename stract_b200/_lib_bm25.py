@@ -87,6 +87,20 @@ class OpticBatch(C.Structure):
                 ("rule_docset", C.c_void_p), ("rule_boost", C.c_void_p), ("exclude", C.c_void_p), ("require", C.c_void_p)]
 
 
+class WebpageBatch(C.Structure):
+    _fields_ = [("n_queries", C.c_uint32), ("n_docs_max", C.c_uint32), ("docs", C.c_void_p), ("n_docs", C.c_void_p),
+                ("dist_field", C.c_uint32 * 2)]
+
+
+class WebpageOut(C.Structure):
+    _fields_ = [("values", C.c_void_p), ("scores", C.c_void_p), ("boosts", C.c_void_p), ("min_slop", C.c_void_p)]
+
+
+class WebpageStats(C.Structure):
+    _fields_ = [("docs", C.c_uint64), ("docs_with_positions", C.c_uint64), ("positions_decoded", C.c_uint64),
+                ("position_bytes", C.c_uint64), ("ms", C.c_float), ("kernel_ms", C.c_float)]
+
+
 def proto(L, f):
     vp, u32, u64, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int
     f("sb200_segment_create", i32, vp, u64, vp, u32, vp, u32, i32, i32, C.POINTER(vp))
@@ -123,3 +137,5 @@ def proto(L, f):
     f("sb200_recall_plan_docs", i32, C.POINTER(RecallPlanBatch), vp, vp, u64, C.POINTER(PlanStats))
     f("sb200_multi_signal_topk_batch_plan", i32, C.POINTER(MultiSignalBatch), C.POINTER(RecallPlanBatch), C.POINTER(OpticBatch), vp, vp, vp,
       C.POINTER(Bm25Stats))
+    f("sb200_multi_signal_webpages", i32, C.POINTER(MultiSignalBatch), C.POINTER(OpticBatch), C.POINTER(WebpageBatch), C.POINTER(WebpageOut),
+      C.POINTER(WebpageStats))

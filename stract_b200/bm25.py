@@ -420,7 +420,8 @@ class RawSignalTable(SignalTable):
     `columns` = {signal name: raw column} (u64 / f64 / bool arrays as in NUMERIC_SIGNALS); the table's column order is
     CoreSignalEnum order.  `current_timestamp` feeds UpdateTimestamp (SignalComputer::set_current_timestamp), `region_count`
     = (counts per region id, total) feeds Region (RegionCount::score), `selected_region` the query's region boost.
-    `numeric` is the [(name, column, default coefficient)] list SignalComputeOrder / MultiFieldSignalComputer take."""
+    `numeric` is the [(name, column, default coefficient)] list SignalComputeOrder / MultiFieldSignalComputer take; `raw` keeps
+    the raw columns by name (a numeric CoreSignal's SignalCalculation.value, MultiFieldSignalComputer.ranking_webpages)."""
 
     def __init__(self, columns, current_timestamp=None, region_count=None, selected_region=None, device=0):
         self._L = lib()
@@ -448,6 +449,7 @@ class RawSignalTable(SignalTable):
                 if selected_region is not None:
                     arr[i].p0, arr[i].p1 = float(selected_region), 1.0
             self.numeric.append((n, i, coef))
+        self.raw = dict(zip(names, keep))
         self.n_cols = len(names)
         self.max_doc = int(keep[0].size) if keep else 0
         assert all(k.size == self.max_doc for k in keep)
@@ -840,16 +842,9 @@ class MultiFieldSignalComputer:
                 c = self.coefficient(name, coef)
         return c
 
-    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None, optic=None, plan=None):
-        """slot_field / slot_term [n_queries, n_slots]: field index into `self.names` (TextFieldEnum order; 0xFF pads) and the term's ordinal in that
-        field's reader (NO_TERM = the segment does not hold it).  idf comes from the field's own doc_freq
-        (MultiBm25Weight::for_terms), the Bm25F idf from `doc_freq_all_body` [n_queries, n_slots] (WeightCache: the AllBody
-        doc_freq of the token), defaulting to the field's own.  Optic rules: a slot with field | 0x80 is the docset of a rule,
-        `slot_boost` [n_queries, n_slots] holds its boost (negative = downrank): SignalComputer::boosts (mod.rs:471-497).
-        `optic` (OpticTables, e.g. from stract_b200.optic.compile_optics): optic rules as device docsets, with the Discard /
-        DiscardNonMatching filters (sb200_multi_signal_topk_batch_optic); None keeps sb200_multi_signal_topk_batch.
-        `plan` (RecallPlan, e.g. from stract_b200.query_plan.compile_plans): the candidates are each query's plan docset instead
-        of the union of its text slots (sb200_multi_signal_topk_batch_plan); None keeps the union."""
+    def _batch(self, slot_field, slot_term, k, doc_freq_all_body, slot_boost, optic):
+        """The sb200_multi_signal_batch (and sb200_optic_batch, or None) of top_docs_batch / ranking_webpages, plus the arrays they
+        point into (kept alive by the caller)."""
         sf = np.ascontiguousarray(slot_field, np.uint8); st = np.ascontiguousarray(slot_term, np.uint32)
         nq, ns = sf.shape
         idf1 = np.zeros((nq, ns), np.float32); idf2 = np.zeros((nq, ns), np.float32)
@@ -873,7 +868,6 @@ class MultiFieldSignalComputer:
         for i, (name, kind, field, chain, col, coef) in enumerate(self.order.entries):
             ops[i].kind = kind; ops[i].field = self.names.index(field) if field is not None else 0
             ops[i].chain = chain; ops[i].col = col; ops[i].coeff = self.coefficient(name, coef)
-        docs = host_out((nq, k), np.uint32); totals = host_out((nq, k), np.float64); n_out = np.zeros(nq, np.uint32)
         mb = B.MultiSignalBatch()
         mb.n_queries, mb.n_slots = nq, ns
         mb.slot_field, mb.slot_term, mb.slot_idf, mb.slot_idf_f = _p(sf), _p(st), _p(idf1), _p(idf2)
@@ -883,11 +877,9 @@ class MultiFieldSignalComputer:
         mb.k = k
         sbst = None if slot_boost is None else np.ascontiguousarray(slot_boost, np.float64)
         mb.slot_boost = _p(sbst)
-        stt = B.Bm25Stats()
         ob = None
-        if optic is None and plan is None:
-            check(self._L.sb200_multi_signal_topk_batch(C.byref(mb), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
-        elif optic is not None:
+        keep = [sf, st, idf1, idf2, caches, farr, ops, sbst]
+        if optic is not None:
             if len(optic.rules) != nq:
                 raise ValueError(f"optic tables for {len(optic.rules)} queries, batch has {nq}")
             mr = max([len(r) for r in optic.rules] + [1])
@@ -902,18 +894,87 @@ class MultiFieldSignalComputer:
             ob = B.OpticBatch()
             ob.n_docsets, ob.max_rules, ob.docsets = len(optic.docsets), mr, C.cast(darr, C.c_void_p)
             ob.n_rules, ob.rule_docset, ob.rule_boost, ob.exclude, ob.require = _p(nr), _p(rd), _p(rb), _p(ex), _p(rq)
-            if plan is None:
-                check(self._L.sb200_multi_signal_topk_batch_optic(C.byref(mb), C.byref(ob), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+            keep += [nr, rd, rb, ex, rq, darr]
+        self.last_inputs = dict(idf=idf1, idf_f=idf2, caches=caches)
+        return mb, ob, keep
+
+    def top_docs_batch(self, slot_field, slot_term, k, doc_freq_all_body=None, return_stats=False, slot_boost=None, optic=None, plan=None):
+        """slot_field / slot_term [n_queries, n_slots]: field index into `self.names` (TextFieldEnum order; 0xFF pads) and the term's ordinal in that
+        field's reader (NO_TERM = the segment does not hold it).  idf comes from the field's own doc_freq
+        (MultiBm25Weight::for_terms), the Bm25F idf from `doc_freq_all_body` [n_queries, n_slots] (WeightCache: the AllBody
+        doc_freq of the token), defaulting to the field's own.  Optic rules: a slot with field | 0x80 is the docset of a rule,
+        `slot_boost` [n_queries, n_slots] holds its boost (negative = downrank): SignalComputer::boosts (mod.rs:471-497).
+        `optic` (OpticTables, e.g. from stract_b200.optic.compile_optics): optic rules as device docsets, with the Discard /
+        DiscardNonMatching filters (sb200_multi_signal_topk_batch_optic); None keeps sb200_multi_signal_topk_batch.
+        `plan` (RecallPlan, e.g. from stract_b200.query_plan.compile_plans): the candidates are each query's plan docset instead
+        of the union of its text slots (sb200_multi_signal_topk_batch_plan); None keeps the union."""
+        mb, ob, keep = self._batch(slot_field, slot_term, k, doc_freq_all_body, slot_boost, optic)
+        nq = mb.n_queries
+        docs = host_out((nq, k), np.uint32); totals = host_out((nq, k), np.float64); n_out = np.zeros(nq, np.uint32)
+        stt = B.Bm25Stats()
+        if plan is None and ob is None:
+            check(self._L.sb200_multi_signal_topk_batch(C.byref(mb), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
+        elif plan is None:
+            check(self._L.sb200_multi_signal_topk_batch_optic(C.byref(mb), C.byref(ob), _p(docs), _p(totals), _p(n_out), C.byref(stt)))
         if plan is not None:
             if plan.n_queries != nq:
                 raise ValueError(f"plan for {plan.n_queries} queries, batch has {nq}")
-            pb, keep = plan._batch()
+            pb, pkeep = plan._batch()
             check(self._L.sb200_multi_signal_topk_batch_plan(C.byref(mb), C.byref(pb), None if ob is None else C.byref(ob), _p(docs),
                                                              _p(totals), _p(n_out), C.byref(stt)))
-        self.last_inputs = dict(idf=idf1, idf_f=idf2, caches=caches)
         if return_stats:
             return docs, totals, n_out, {k_: getattr(stt, k_) for k_, _ in B.Bm25Stats._fields_ if not k_.startswith("_")}
         return docs, totals, n_out
+
+    def ranking_webpages(self, slot_field, slot_term, docs, n_docs, distance_fields=("Title", "CleanBody"), slot_boost=None, optic=None,
+                         doc_freq_all_body=None, return_stats=False):
+        """What LocalRecallRankingWebpage::new (core/src/ranking/pipeline/stages/recall.rs:167-220) takes from this computer for
+        the documents docs[q, :n_docs[q]] of every query (any order, repeats allowed; outputs follow it), with the slots, ops and
+        optic rules of top_docs_batch (sb200_multi_signal_webpages):
+          names     the op entries' signal names (self.order.entries order)
+          values / scores [n_queries, n_docs_max, n_ops] f64  each op's SignalCalculation: text signals value before, score after
+                    n-gram dampening; a numeric signal's value is its raw column as f64 when self.signals is a RawSignalTable, NaN
+                    with a plain SignalTable (it holds scores only)
+          boosts    [n_queries, n_docs_max]  SignalComputer::boosts, 1.0 without rules (the exclude / require filters are not applied)
+          min_slop  [n_queries, n_docs_max, 2] u32  term_distance.rs min_slop over `distance_fields` (u32::MAX when a field is not
+                    among self.names, has < 2 slots, or a slot lacks the document)
+        Entries past n_docs[q] are 0 (values NaN)."""
+        docs = np.ascontiguousarray(docs, np.uint32)
+        nd_ = np.ascontiguousarray(n_docs, np.uint32)
+        nq, ndm = docs.shape
+        mb, ob, keep = self._batch(slot_field, slot_term, 0, doc_freq_all_body, slot_boost, optic)
+        n_ops = len(self.order.entries)
+        values = np.full((nq, ndm, n_ops), np.nan); scores = np.zeros((nq, ndm, n_ops)); boosts = np.zeros((nq, ndm))
+        min_slop = np.zeros((nq, ndm, 2), np.uint32)
+        wb = B.WebpageBatch()
+        wb.n_queries, wb.n_docs_max, wb.docs, wb.n_docs = nq, ndm, _p(docs), _p(nd_)
+        for i, name in enumerate(distance_fields):
+            wb.dist_field[i] = self.names.index(name) if name in self.names else WEBPAGE_NO_FIELD
+        out = B.WebpageOut()
+        out.values, out.scores, out.boosts, out.min_slop = _p(values), _p(scores), _p(boosts), _p(min_slop)
+        stt = B.WebpageStats()
+        check(self._L.sb200_multi_signal_webpages(C.byref(mb), None if ob is None else C.byref(ob), C.byref(wb), C.byref(out), C.byref(stt)))
+        raw = getattr(self.signals, "raw", None)
+        if raw is not None:
+            live = np.arange(ndm)[None, :] < nd_[:, None]
+            for o, (name, kind, _f, _c, _col, _coef) in enumerate(self.order.entries):
+                if kind == OP_NUMERIC and name in raw:
+                    values[:, :, o] = np.where(live, raw[name][np.where(live, docs, 0)].astype(np.float64), np.nan)
+        res = RankingWebpages([e[0] for e in self.order.entries], values, scores, boosts, min_slop)
+        if return_stats:
+            return res, {k_: getattr(stt, k_) for k_, _ in B.WebpageStats._fields_}
+        return res
+
+
+WEBPAGE_NO_FIELD = 0xFFFFFFFF
+
+
+class RankingWebpages:
+    """MultiFieldSignalComputer.ranking_webpages' result: `names` of the ops, `values` / `scores` [n_queries, n_docs_max, n_ops],
+    `boosts` [n_queries, n_docs_max], `min_slop` [n_queries, n_docs_max, 2] (Title, CleanBody)."""
+
+    def __init__(self, names, values, scores, boosts, min_slop):
+        self.names, self.values, self.scores, self.boosts, self.min_slop = names, values, scores, boosts, min_slop
 
 
 # ---------------------------------------------------------------------------------------------- query-plan recall docset ----

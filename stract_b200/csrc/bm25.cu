@@ -23,6 +23,7 @@
 //   optic pattern docsets k_phrase_cand + k_pattern_verify and word kernels (bm25_pattern.cuh); k_sig_multi<TMAX, true>
 //                        consumes them in the recall stage.
 //   query-plan docsets   k_plan_cover + CUB sort + k_plan_eval + CUB select (bm25_plan.cuh); k_plan_recall scores them.
+//   recall webpages      CUB sort + k_wp_signals + k_wp_slop (bm25_webpage.cuh): signals, boosts and term distances of given docs.
 // A query of the walk kernels much larger than the batch average is cut into doc-range work items (plan_items);
 // k_merge_topk merges their partial top-k lists.  Keys are (order-preserving score bits, ~doc), so the result order
 // is the reference's (score desc, doc asc) total order.
@@ -108,6 +109,11 @@ struct sb200_segment {
   sb200::DevBuf<uint8_t> pl_segs, pl_nodes, pl_cover, pl_keep, pl_tmp;
   sb200::DevBuf<uint64_t> pl_keys, pl_keys2, pl_beg, pl_cnt;
   sb200::DevBuf<uint32_t> pl_off, pl_units, pl_ph_off, pl_ph_docs;
+  // scratch of the recall webpages (bm25_webpage.cuh; in the first field's handle)
+  sb200::DevBuf<uint64_t> wp_keys, wp_keys2, wp_off, wp_work, wp_ovl, wp_ovc;
+  sb200::DevBuf<uint32_t> wp_idx, wp_idx2, wp_beg, wp_units, wp_tf, wp_slop, wp_scratch;
+  sb200::DevBuf<double> wp_values, wp_scores, wp_boosts;
+  sb200::DevBuf<uint8_t> wp_tmp;
 };
 
 struct sb200_docset {
@@ -274,6 +280,7 @@ static int launch_topk_warp(const WParams& P, cudaStream_t s) {
 #include "bm25_phrase.cuh"
 #include "bm25_pattern.cuh"
 #include "bm25_plan.cuh"
+#include "bm25_webpage.cuh"
 #include <chrono>
 #include <functional>
 namespace sb200 {
@@ -336,16 +343,21 @@ static int launch_plan_recall(const PlanRecallParams& R, cudaStream_t s) {
   return SB200_OK;
 }
 
-// pb != NULL: the candidates are each query's plan docset (run_plan) instead of the union of its text slots
+struct WpCall { const sb200_webpage_batch* b; const sb200_webpage_out* out; sb200_webpage_stats* stats; };
+static int run_webpages(sb200_segment* g, const MParams& P, const sb200_multi_signal_batch* b, const std::vector<uint8_t>& sf,
+                        const std::vector<uint32_t>& ns, const WpCall& wp);
+
+// pb != NULL: the candidates are each query's plan docset (run_plan) instead of the union of its text slots.  wp != NULL: no
+// top-k; the signals, boosts and term distances of the caller's documents (run_webpages).
 static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch* ob, uint32_t* docs, double* totals, uint32_t* n_out,
-                     sb200_bm25_stats* stats, const sb200_recall_plan_batch* pb = nullptr) {
-  if (!b || !b->fields || !b->ops || !b->slot_field || !b->slot_term || !b->slot_idf || !b->slot_idf_f || !docs || !totals || !n_out)
+                     sb200_bm25_stats* stats, const sb200_recall_plan_batch* pb = nullptr, const WpCall* wp = nullptr) {
+  if (!b || !b->fields || !b->ops || !b->slot_field || !b->slot_term || !b->slot_idf || !b->slot_idf_f || (!wp && (!docs || !totals || !n_out)))
     SB_FAIL(SB200_EINVAL, "NULL argument");
   const uint32_t nq = b->n_queries, SM = b->n_slots, k = b->k, NF = b->n_fields, NO = b->n_ops;
   if (NF == 0 || NF > (uint32_t)M_MAX_FIELDS) SB_FAIL(SB200_ERANGE, "n_fields %u outside [1,%d]", NF, M_MAX_FIELDS);
   if (NO == 0 || NO > (uint32_t)M_MAX_OPS) SB_FAIL(SB200_ERANGE, "n_ops %u outside [1,%d]", NO, M_MAX_OPS);
   if (SM == 0 || SM > 16) SB_FAIL(SB200_ERANGE, "n_slots %u outside [1,16]", SM);
-  if (k == 0 || k > SB200_MAX_K) SB_FAIL(SB200_ERANGE, "k %u outside [1,%d]", k, SB200_MAX_K);
+  if (!wp && (k == 0 || k > SB200_MAX_K)) SB_FAIL(SB200_ERANGE, "k %u outside [1,%d]", k, SB200_MAX_K);
   sb200_segment* g = b->fields[0].seg;
   if (!g) SB_FAIL(SB200_EINVAL, "field 0 has no segment");
   SB_CUDA(cudaSetDevice(g->device));
@@ -414,7 +426,7 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     }
     postings += work[q];
   }
-  if (!pb) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t c) { return work[a] > work[c]; });
+  if (!pb && !wp) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t c) { return work[a] > work[c]; });
   for (uint32_t slot = 0; slot < nq; slot++) {
     const uint32_t q = order[slot];
     uint32_t c = 0;
@@ -430,7 +442,7 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     ns[slot] = c; work_sorted[slot] = work[q];
   }
   ItemPlan pl;   // the plan path has its own work items (one per query, k_plan_recall) and candidate buffers
-  if (!pb) plan_items(work_sorted, order, k, g->max_doc, true, pl);
+  if (!pb && !wp) plan_items(work_sorted, order, k, g->max_doc, true, pl);
   const uint32_t n_items = (uint32_t)pl.q.size();
   const size_t n_slots_out = (size_t)nq + pl.extra;
   uint32_t cap = 1024; while (cap < k + SM * 128u) cap <<= 1;
@@ -500,6 +512,7 @@ static int run_multi(const sb200_multi_signal_batch* b, const sb200_optic_batch*
     P.d_bits = (const uint32_t* const*)g->o_bits.p; P.d_nrules = g->o_nrules.p; P.d_rule = g->o_rule.p; P.d_boost = g->o_boost.p;
     P.d_max_rules = MR; P.d_exclude = g->o_exclude.p; P.d_require = g->o_require.p;
   }
+  if (wp) return run_webpages(g, P, b, sf, ns, *wp);
   if (pb) {   // the plan docset group by group; each group's recall runs on this stream once its docset is complete
     SB_CUDA(cudaStreamSynchronize(s));
     uint32_t rcap = 1024; while (rcap < k + 32) rcap <<= 1;
@@ -1009,6 +1022,147 @@ static int phrase_match(sb200_segment* g, uint32_t nq, uint32_t nt, const std::v
     }
     SB_TRY(done(g0, g1));
     g0 = g1;
+  }
+  return SB200_OK;
+}
+
+template <int TMAX>
+static int launch_wp_signals(const WpParams& W, cudaStream_t s) {
+  const size_t sm = wp_cta_smem<TMAX>();
+  static bool configured = false;
+  if (!configured) { SB_CUDA(cudaFuncSetAttribute(k_wp_signals<TMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); configured = true; }
+  SB_LAUNCH(k_wp_signals<TMAX>, div_up(W.n_units, WQ), WQ * 32, sm, s, W);
+  SB_CHECK_LAUNCH();
+  return SB200_OK;
+}
+
+// Recall webpages (bm25_webpage.cuh) of the caller's documents, after run_multi uploaded the slots (query order kept, text slots
+// first) and the optic tables: sort, k_wp_signals, then k_wp_slop over the (document, distance field) pairs that need positions --
+// a shared-memory pass and a global-scratch pass for the pairs whose lists do not fit.  sb200_multi_signal_webpages checked wp.b.
+static int run_webpages(sb200_segment* g, const MParams& P, const sb200_multi_signal_batch* b, const std::vector<uint8_t>& sf,
+                        const std::vector<uint32_t>& ns, const WpCall& wp) {
+  const sb200_webpage_batch* wb = wp.b;
+  const sb200_webpage_out* out = wp.out;
+  cudaStream_t s = g->stream;
+  const uint32_t nq = wb->n_queries, ndm = wb->n_docs_max, SM = b->n_slots, NO = b->n_ops;
+  const size_t n_out = (size_t)nq * ndm;
+  // keys in the caller's order, each query's range and its 32-key chunks
+  std::vector<uint32_t> beg(nq + 1, 0), units;
+  for (uint32_t q = 0; q < nq; q++) beg[q + 1] = beg[q] + wb->n_docs[q];
+  const uint32_t n_keys = beg[nq];
+  std::vector<uint64_t> keys(n_keys);
+  std::vector<uint32_t> idx(n_keys);
+  for (uint32_t q = 0; q < nq; q++) {
+    for (uint32_t i = 0; i < wb->n_docs[q]; i++) {
+      keys[beg[q] + i] = ((uint64_t)q << 32) | wb->docs[(size_t)q * ndm + i];
+      idx[beg[q] + i] = (uint32_t)((size_t)q * ndm + i);
+    }
+    for (uint32_t c = 0; c < wb->n_docs[q]; c += 32) units.push_back(beg[q] + c);
+  }
+  // row width of the offset scratch: the distance fields' text slots of a query, at most
+  uint32_t nd = 1;
+  for (uint32_t q = 0; q < nq; q++) {
+    uint32_t c = 0;
+    for (uint32_t x = 0; x < ns[q]; x++) { const uint8_t f = sf[(size_t)q * SM + x]; if (f == wb->dist_field[0] || f == wb->dist_field[1]) c++; }
+    nd = std::max(nd, c);
+  }
+  const size_t nk = std::max<size_t>(n_keys, 1);
+  SB_TRY(ensure(g->wp_keys, nk)); SB_TRY(ensure(g->wp_keys2, nk)); SB_TRY(ensure(g->wp_idx, nk)); SB_TRY(ensure(g->wp_idx2, nk));
+  SB_TRY(ensure(g->wp_beg, nq + 1)); SB_TRY(ensure(g->wp_units, std::max<size_t>(units.size(), 1)));
+  SB_TRY(ensure(g->wp_off, nk * nd)); SB_TRY(ensure(g->wp_tf, nk * nd)); SB_TRY(ensure(g->wp_work, 2 * nk)); SB_TRY(ensure(g->wp_ovl, 2 * nk));
+  SB_TRY(ensure(g->wp_ovc, 4)); SB_TRY(ensure(g->counters, 8));
+  const size_t no = std::max<size_t>(n_out, 1);
+  SB_TRY(ensure(g->wp_values, no * NO)); SB_TRY(ensure(g->wp_scores, no * NO)); SB_TRY(ensure(g->wp_boosts, no)); SB_TRY(ensure(g->wp_slop, no * 2));
+  float kms = 0.0f;
+  auto timed = [&](auto&& launch) -> int {
+    SB_CUDA(cudaEventRecord(g->evk0, s));
+    SB_TRY(launch());
+    SB_CUDA(cudaEventRecord(g->evk1, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.0f; cudaEventElapsedTime(&ms, g->evk0, g->evk1); kms += ms;
+    return SB200_OK;
+  };
+  if (n_out) {   // values of the numeric ops are not written: keep the caller's
+    SB_CUDA(cudaMemcpyAsync(g->wp_values.p, out->values, n_out * NO * 8, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemsetAsync(g->wp_scores.p, 0, n_out * NO * 8, s));
+    SB_CUDA(cudaMemsetAsync(g->wp_boosts.p, 0, n_out * 8, s));
+    SB_CUDA(cudaMemsetAsync(g->wp_slop.p, 0, n_out * 8, s));
+  }
+  SB_CUDA(cudaMemsetAsync(g->counters.p, 0, 8 * sizeof(unsigned long long), s));
+  SB_CUDA(cudaMemsetAsync(g->wp_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+  unsigned long long h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (n_keys) {
+    SB_CUDA(cudaMemcpyAsync(g->wp_keys.p, keys.data(), (size_t)n_keys * 8, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->wp_idx.p, idx.data(), (size_t)n_keys * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->wp_beg.p, beg.data(), (size_t)(nq + 1) * 4, cudaMemcpyHostToDevice, s));
+    SB_CUDA(cudaMemcpyAsync(g->wp_units.p, units.data(), units.size() * 4, cudaMemcpyHostToDevice, s));
+    int qbits = 1; while ((1ull << qbits) < nq) qbits++;
+    cub::DoubleBuffer<uint64_t> dk((uint64_t*)g->wp_keys.p, (uint64_t*)g->wp_keys2.p);
+    cub::DoubleBuffer<uint32_t> dv(g->wp_idx.p, g->wp_idx2.p);
+    size_t need = 0;
+    SB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, need, dk, dv, (int64_t)n_keys, 0, 32 + qbits, s));
+    SB_TRY(ensure(g->wp_tmp, need + 256));
+    SB_TRY(timed([&]() -> int { SB_CUDA(cub::DeviceRadixSort::SortPairs(g->wp_tmp.p, need, dk, dv, (int64_t)n_keys, 0, 32 + qbits, s)); return SB200_OK; }));
+    WpParams W;
+    memset(&W, 0, sizeof(W));
+    W.M = P;
+    W.keys = dk.Current(); W.idx = dv.Current(); W.q_beg = g->wp_beg.p; W.units = g->wp_units.p; W.n_units = (uint32_t)units.size();
+    for (int f = 0; f < 2; f++) {
+      W.dist[f] = wb->dist_field[f];
+      W.pos_base[f] = wb->dist_field[f] == SB200_WEBPAGE_NO_FIELD ? nullptr : b->fields[wb->dist_field[f]].seg->pos_base.p;
+    }
+    W.nd = nd; W.s_off = g->wp_off.p; W.s_tf = g->wp_tf.p;
+    W.o_values = g->wp_values.p; W.o_scores = g->wp_scores.p; W.o_boosts = g->wp_boosts.p; W.o_slop = g->wp_slop.p;
+    W.work = (unsigned long long*)g->wp_work.p; W.counters = g->counters.p;
+    SB_TRY(timed([&]() -> int { if (SM <= 8) return launch_wp_signals<8>(W, s); return launch_wp_signals<16>(W, s); }));
+    SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    SB_CUDA(cudaStreamSynchronize(s));
+    if (h[1]) SB_FAIL(SB200_EFORMAT, "%llu chunks met inconsistent posting data", h[1]);
+    if (h[0]) {
+      int n_sm = 132;
+      { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 132; }
+      WpSlopParams Q;
+      memset(&Q, 0, sizeof(Q));
+      for (int f = 0; f < 2; f++) {
+        Q.dist[f] = wb->dist_field[f];
+        if (wb->dist_field[f] != SB200_WEBPAGE_NO_FIELD) pos_view(b->fields[wb->dist_field[f]].seg, Q.V[f]);
+      }
+      Q.keys = W.keys; Q.idx = W.idx;
+      Q.q_slot_field = P.q_slot_field; Q.q_slot_term = P.q_slot_term; Q.q_nslots = P.q_nslots; Q.n_slots_max = SM;
+      Q.nd = nd; Q.s_off = g->wp_off.p; Q.s_tf = g->wp_tf.p;
+      Q.work = W.work; Q.n = h[0];
+      Q.ov_list = (unsigned long long*)g->wp_ovl.p; Q.ov = (unsigned long long*)g->wp_ovc.p; Q.scratch_cursor = Q.ov + 2;
+      Q.o_slop = g->wp_slop.p; Q.counters = g->counters.p;
+      const unsigned grid = (unsigned)std::min<uint64_t>(div_up(h[0], PH_WARPS), (uint64_t)n_sm * 16);
+      SB_TRY(timed([&]() -> int { SB_LAUNCH(k_wp_slop, grid, PH_WARPS * 32, 0, s, Q); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      unsigned long long ov[4] = {0, 0, 0, 0};
+      SB_CUDA(cudaMemcpyAsync(ov, g->wp_ovc.p, sizeof(ov), cudaMemcpyDeviceToHost, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      if (ov[0]) {   // the lists of these pairs do not fit shared memory: one pass over global scratch sized by their total
+        SB_TRY(ensure(g->wp_scratch, (size_t)ov[1] + 64));
+        SB_CUDA(cudaMemcpyAsync(g->wp_work.p, g->wp_ovl.p, ov[0] * 8, cudaMemcpyDeviceToDevice, s));
+        SB_CUDA(cudaMemsetAsync(g->wp_ovc.p, 0, 4 * sizeof(unsigned long long), s));
+        Q.work = (const unsigned long long*)g->wp_work.p; Q.n = ov[0]; Q.scratch = g->wp_scratch.p;
+        const unsigned grid2 = (unsigned)std::min<uint64_t>(div_up(ov[0], PH_WARPS), (uint64_t)n_sm * 16);
+        SB_TRY(timed([&]() -> int { SB_LAUNCH(k_wp_slop, grid2, PH_WARPS * 32, 0, s, Q); SB_CHECK_LAUNCH(); return SB200_OK; }));
+      }
+      SB_CUDA(cudaMemcpyAsync(h, g->counters.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+      SB_CUDA(cudaStreamSynchronize(s));
+      if (h[1]) SB_FAIL(SB200_EFORMAT, "%llu documents met inconsistent posting or positions data", h[1]);
+    }
+  }
+  if (n_out) {
+    SB_CUDA(cudaMemcpyAsync(out->values, g->wp_values.p, n_out * NO * 8, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemcpyAsync(out->scores, g->wp_scores.p, n_out * NO * 8, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemcpyAsync(out->boosts, g->wp_boosts.p, n_out * 8, cudaMemcpyDefault, s));
+    SB_CUDA(cudaMemcpyAsync(out->min_slop, g->wp_slop.p, n_out * 8, cudaMemcpyDefault, s));
+  }
+  SB_CUDA(cudaEventRecord(g->ev1, s));
+  SB_CUDA(cudaStreamSynchronize(s));
+  if (wp.stats) {
+    float ms = 0; cudaEventElapsedTime(&ms, g->ev0, g->ev1);
+    wp.stats->docs = n_keys; wp.stats->docs_with_positions = h[2]; wp.stats->positions_decoded = h[3]; wp.stats->position_bytes = h[4];
+    wp.stats->ms = ms; wp.stats->kernel_ms = kms;
   }
   return SB200_OK;
 }
@@ -2154,6 +2308,35 @@ int sb200_multi_signal_topk_batch_plan(const sb200_multi_signal_batch* batch, co
                                        uint32_t* docs, double* totals, uint32_t* n_out, sb200_bm25_stats* stats) {
   if (!plan) SB_FAIL(SB200_EINVAL, "NULL plan batch");
   return run_multi(batch, optic, docs, totals, n_out, stats, plan);
+}
+
+int sb200_multi_signal_webpages(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, const sb200_webpage_batch* wb,
+                                const sb200_webpage_out* out, sb200_webpage_stats* stats) {
+  using namespace sb200;
+  if (!batch || !batch->fields || !wb || !out) SB_FAIL(SB200_EINVAL, "NULL argument");
+  if (wb->n_queries != batch->n_queries) SB_FAIL(SB200_EINVAL, "webpage batch has %u queries, signal batch %u", wb->n_queries, batch->n_queries);
+  const uint32_t NF = batch->n_fields, nq = wb->n_queries, ndm = wb->n_docs_max;
+  if (NF == 0 || NF > (uint32_t)M_MAX_FIELDS) SB_FAIL(SB200_ERANGE, "n_fields %u outside [1,%d]", NF, M_MAX_FIELDS);
+  if ((uint64_t)nq * ndm > 0xFFFFFFFFull) SB_FAIL(SB200_ERANGE, "n_queries * n_docs_max = %llu above 2^32 - 1", (unsigned long long)nq * ndm);
+  if (nq && (!wb->n_docs || (ndm && !wb->docs))) SB_FAIL(SB200_EINVAL, "NULL docs / n_docs");
+  if (nq && ndm && (!out->values || !out->scores || !out->boosts || !out->min_slop)) SB_FAIL(SB200_EINVAL, "NULL output");
+  const sb200_segment* g0 = batch->fields[0].seg;
+  if (!g0) SB_FAIL(SB200_EINVAL, "field 0 has no segment");
+  for (int f = 0; f < 2; f++) {
+    const uint32_t x = wb->dist_field[f];
+    if (x == SB200_WEBPAGE_NO_FIELD) continue;
+    if (x >= NF) SB_FAIL(SB200_EINVAL, "distance field %d: field index %u >= %u", f, x, NF);
+    if (!batch->fields[x].seg || !batch->fields[x].seg->has_pos) SB_FAIL(SB200_EINVAL, "distance field %d (field %u) has no positions attached", f, x);
+  }
+  if (wb->dist_field[0] != SB200_WEBPAGE_NO_FIELD && wb->dist_field[0] == wb->dist_field[1]) SB_FAIL(SB200_EINVAL, "both distance fields are field %u", wb->dist_field[0]);
+  for (uint32_t q = 0; q < nq; q++) {
+    if (wb->n_docs[q] > ndm) SB_FAIL(SB200_EINVAL, "query %u: n_docs %u > n_docs_max %u", q, wb->n_docs[q], ndm);
+    for (uint32_t i = 0; i < wb->n_docs[q]; i++)
+      if (wb->docs[(size_t)q * ndm + i] >= g0->max_doc) SB_FAIL(SB200_EINVAL, "query %u doc %u: %u >= max_doc %u", q, i, wb->docs[(size_t)q * ndm + i], g0->max_doc);
+  }
+  const WpCall wp{wb, out, stats};
+  if (stats) memset(stats, 0, sizeof(*stats));
+  return run_multi(batch, optic, nullptr, nullptr, nullptr, nullptr, nullptr, &wp);
 }
 
 int sb200_multi_signal_topk_batch_optic(const sb200_multi_signal_batch* batch, const sb200_optic_batch* optic, uint32_t* docs,

@@ -61,13 +61,23 @@ __host__ __device__ constexpr size_t m_warp_smem() { return (size_t)TMAX * 128 *
 template <int TMAX>
 __host__ __device__ constexpr size_t m_cta_smem() { return M_MAX_FIELDS * 256 * 4 + M_MAX_OPS * sizeof(MOp) + WQ * m_warp_smem<TMAX>(); }
 
+// What m_total reports besides the total: every op's (value before n-gram dampening, score after it) and every boost factor
+// it multiplies the total with.  The top-k kernels pass MNoSink (ACTIVE = false: m_total compiles exactly as without a sink);
+// k_wp_signals (bm25_webpage.cuh) keeps them.
+struct MNoSink {
+  static constexpr bool ACTIVE = false;
+  __device__ __forceinline__ void op(const MOp&, uint32_t, double, double) {}
+  __device__ __forceinline__ void boost(double) {}
+};
+
 // The per-candidate signal program of one document with the term frequencies of its T slots known (tf 0 = the slot does not
-// hold it): the ops in order, the rule-slot boosts, then (OPTIC) the docset-rule boosts.  k_sig_multi and k_plan_recall
-// (bm25_plan.cuh) both call it, so a document gets the same f64 total whichever kernel found it.
-template <int TMAX, bool OPTIC>
+// hold it): the ops in order, the rule-slot boosts, then (OPTIC) the docset-rule boosts.  k_sig_multi, k_plan_recall
+// (bm25_plan.cuh) and k_wp_signals (bm25_webpage.cuh) all call it, so a document gets the same f64 total whichever kernel
+// found it.
+template <int TMAX, bool OPTIC, class SINK>
 __device__ __forceinline__ double m_total(const MParams& P, const MOp* s_ops, const float* s_cache, const uint32_t* s_nf, const uint32_t* s_fld,
                                           const float* s_wf, const OTerm* tc, uint32_t T, uint32_t q, uint32_t d, const uint32_t (&tf)[TMAX],
-                                          uint32_t o_q, uint32_t o_nr) {
+                                          uint32_t o_q, uint32_t o_nr, SINK& sink) {
   const uint32_t SM = P.n_slots_max;
   const double DAMP[3] = {1.0, 0.4, 0.4 * 0.4};   // NGRAM_DAMPENING.powi(hits) (order.rs:99,127)
   uint32_t fid[M_MAX_FIELDS];
@@ -120,11 +130,14 @@ __device__ __forceinline__ double m_total(const MParams& P, const MOp* s_ops, co
         sc = (double)b;
       }
     }
+    double value = 0.0;
+    if constexpr (SINK::ACTIVE) value = sc;
     if (op.chain) {
       if (op.chain == 1u) hits = 0;
       sc = __dmul_rn(sc, DAMP[hits > 2 ? 2 : hits]);
       if (sc > 0.0) hits++;
     }
+    if constexpr (SINK::ACTIVE) sink.op(op, o, value, sc);
     total = __dadd_rn(total, __dmul_rn(op.coeff, sc));
   }
   if (P.q_boost) {   // SignalComputer::boosts
@@ -135,6 +148,7 @@ __device__ __forceinline__ double m_total(const MParams& P, const MOp* s_ops, co
       if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
     }
     const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
+    if constexpr (SINK::ACTIVE) sink.boost(factor);
     total = __dmul_rn(total, factor);
   }
   if constexpr (OPTIC) {
@@ -147,6 +161,7 @@ __device__ __forceinline__ double m_total(const MParams& P, const MOp* s_ops, co
         if (b < 0.0) down = __dadd_rn(down, fabs(b)); else up = __dadd_rn(up, b);
       }
       const double factor = (down > up) ? __ddiv_rn(1.0, __dadd_rn(1.0, __dsub_rn(down, up))) : __dadd_rn(__dsub_rn(up, down), 1.0);
+      if constexpr (SINK::ACTIVE) sink.boost(factor);
       total = __dmul_rn(total, factor);
     }
   }
@@ -323,7 +338,8 @@ __global__ void __launch_bounds__(WQ * 32) k_sig_multi(const MParams P) {
         if (o_rq && !m_in(o_rq, d)) continue;   // DiscardNonMatching
       }
       my_docs++;
-      const double total = m_total<TMAX, OPTIC>(P, s_ops, s_cache, s_nf, s_fld, s_wf, tc, T, q, d, tf, o_q, o_nr);
+      MNoSink none;
+      const double total = m_total<TMAX, OPTIC>(P, s_ops, s_cache, s_nf, s_fld, s_wf, tc, T, q, d, tf, o_q, o_nr, none);
       const uint64_t kh = ord_f64(total);
       const uint32_t kl = ~d;
       if (thr_on && !key_gt(kh, kl, thr_hi, thr_lo)) continue;

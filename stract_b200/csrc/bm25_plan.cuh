@@ -45,9 +45,16 @@ __device__ __forceinline__ OTerm pl_term(const PSeg& G, uint32_t ord) {
 // frequency, 0 when the term does not hold d, or PL_BAD when the directory and the block contents disagree.  *cur / *cached
 // (shared memory) are the warp's cursor -- a block index that only moves forward -- and the block held in docs / tfs; they
 // persist between calls for the same term.
+// POS observes the seek: block(tfs, lane) after every block decode (the whole warp), hit(j, jj) when a lane finds d at entry jj
+// of block j.  pl_seek itself observes nothing; k_wp_signals (bm25_webpage.cuh) records position offsets this way.
 constexpr uint64_t PL_BAD = 1ull << 32;
-__device__ uint64_t pl_seek(const PSeg& G, const OTerm& c, uint32_t* cur_p, uint32_t* cached_p, uint32_t* docs, uint32_t* tfs, uint32_t* bloom,
-                            uint32_t d, bool want, uint32_t lane) {
+struct PlNoPos {
+  __device__ __forceinline__ void block(const uint32_t*, uint32_t) {}
+  __device__ __forceinline__ void hit(uint32_t, uint32_t) {}
+};
+template <class POS>
+__device__ __forceinline__ uint64_t pl_seek_at(const PSeg& G, const OTerm& c, uint32_t* cur_p, uint32_t* cached_p, uint32_t* docs, uint32_t* tfs,
+                                               uint32_t* bloom, uint32_t d, bool want, uint32_t lane, POS& pos) {
   uint32_t cur = *cur_p, cached = *cached_p, tf = 0;
   bool pend = want && c.df > 0, bad = false;
   for (uint32_t guard = 0;; guard++) {
@@ -63,18 +70,24 @@ __device__ uint64_t pl_seek(const PSeg& G, const OTerm& c, uint32_t* cur_p, uint
       o3_decode(G.S, G.a128, c, j, prev, docs, tfs, bloom, lane, last);
       cached = j;
       __syncwarp();
+      pos.block(tfs, lane);
     }
     const uint32_t lastB = j < c.nfull ? docs[127] : 0xFFFFFFFFu;   // the tail decides everything that is left
     if (pend && d <= lastB) {
       pend = false;
       const uint32_t jj = lower_bound128(docs, d);
-      if (jj < 128u && docs[jj] == d) tf = tfs[jj];
+      if (jj < 128u && docs[jj] == d) { tf = tfs[jj]; pos.hit(j, jj); }
     }
   }
   __syncwarp();
   if (lane == 0) { *cur_p = cur; *cached_p = cached; }
   __syncwarp();
   return bad ? PL_BAD : (uint64_t)tf;
+}
+__device__ uint64_t pl_seek(const PSeg& G, const OTerm& c, uint32_t* cur_p, uint32_t* cached_p, uint32_t* docs, uint32_t* tfs, uint32_t* bloom,
+                            uint32_t d, bool want, uint32_t lane) {
+  PlNoPos none;
+  return pl_seek_at(G, c, cur_p, cached_p, docs, tfs, bloom, d, want, lane, none);
 }
 
 struct PlanParams {
@@ -288,7 +301,8 @@ __global__ void __launch_bounds__(WQ * 32) k_plan_recall(const PlanRecallParams 
     }
     if (take) {
       my_docs++;
-      const double total = m_total<TMAX, true>(P, s_ops, s_cache, s_nf, s_fld, s_wf, tc, T, q, d, tf, oq, o_nr);
+      MNoSink none;
+      const double total = m_total<TMAX, true>(P, s_ops, s_cache, s_nf, s_fld, s_wf, tc, T, q, d, tf, oq, o_nr, none);
       const uint64_t kh = ord_f64(total);
       const uint32_t kl = ~d;
       if (!thr_on || key_gt(kh, kl, thr_hi, thr_lo)) {

@@ -1,0 +1,143 @@
+"""Host mirror of Stract's recall ranking stage (RankingPipeline::recall_stage, core/src/ranking/pipeline/stages/recall.rs:303-333,
+pipeline/mod.rs:136-162) over the recall webpages of MultiFieldSignalComputer.ranking_webpages.
+
+A page is (signals, score, boost): `signals` maps a SignalEnum name to (value, score); the page starts with the initial total
+as its score and SignalComputer::boosts as its boost (recall.rs:198-217).  Each stage computes, then `update_scores` re-sums
+sum(score * coefficient) over the present signals in SignalEnum order (scorers/mod.rs:50-56), then `rank` sorts the pages
+stably by boost * score, descending.  The InboundSimilarity modifier multiplies the boost by value + 8 and re-ranks without
+re-summing.  LambdaMART, the embeddings themselves and the precision stage need models and are not mirrored."""
+import numpy as np
+
+from .bm25 import CORE_SIGNALS, NUMERIC_SIGNALS
+
+# SignalEnum in declaration order (core/src/ranking/signals/mod.rs:108-155): the iteration order of EnumMap<SignalEnum, _>
+SIGNAL_ENUM = ["Bm25F", "Bm25Title", "TitleCoverage", "Bm25TitleBigrams", "Bm25TitleTrigrams", "Bm25CleanBody", "CleanBodyCoverage",
+               "Bm25CleanBodyBigrams", "Bm25CleanBodyTrigrams", "Bm25StemmedTitle", "Bm25StemmedCleanBody", "Bm25AllBody", "Bm25Keywords",
+               "Bm25BacklinkText", "IdfSumUrl", "IdfSumSite", "IdfSumDomain", "IdfSumSiteNoTokenizer", "IdfSumDomainNoTokenizer",
+               "IdfSumDomainNameNoTokenizer", "IdfSumDomainIfHomepage", "IdfSumDomainNameIfHomepageNoTokenizer",
+               "IdfSumDomainIfHomepageNoTokenizer", "IdfSumTitleIfHomepage", "CrossEncoderSnippet", "CrossEncoderTitle", "HostCentrality",
+               "HostCentralityRank", "PageCentrality", "PageCentralityRank", "IsHomepage", "FetchTimeMs", "UpdateTimestamp",
+               "TrackerScore", "Region", "QueryCentrality", "InboundSimilarity", "LambdaMart", "UrlDigits", "UrlSlashes", "LinkDensity",
+               "TitleEmbeddingSimilarity", "KeywordEmbeddingSimilarity", "HasAds", "MinTitleSlop", "MinCleanBodySlop"]
+
+# default coefficients of the signals outside CoreSignalEnum (core/src/ranking/signals/non_core/*.rs)
+NON_CORE_COEFFICIENTS = {"QueryCentrality": 0.0, "InboundSimilarity": 0.25, "LambdaMart": 10.0, "MinTitleSlop": 0.1, "MinCleanBodySlop": 0.1,
+                         "CrossEncoderSnippet": 0.17, "CrossEncoderTitle": 0.17, "TitleEmbeddingSimilarity": 0.01,
+                         "KeywordEmbeddingSimilarity": 0.01}
+
+U32_MAX = 0xFFFFFFFF
+INBOUND_SIMILARITY_SMOOTHING = 8.0   # modifiers/inbound_similarity.rs
+
+
+def default_coefficients():
+    """SignalCoefficients::default(): every SignalEnum's default coefficient."""
+    c = {name: coef for name, _k, _f, _s, coef in CORE_SIGNALS}
+    c.update({name: coef for name, _k, _d, coef in NUMERIC_SIGNALS})
+    c.update(NON_CORE_COEFFICIENTS)
+    return c
+
+
+def min_slop_two_positions(pos_a, pos_b):
+    """term_distance.rs:23-46, the two-cursor walk"""
+    cur_min, ca, cb = U32_MAX, 0, 0
+    while ca < len(pos_a) and cb < len(pos_b):
+        a, b = pos_a[ca], pos_b[cb]
+        if b > a:
+            cur_min = min(b - a, cur_min)
+            ca += 1
+        else:
+            cb += 1
+    return cur_min
+
+
+def min_slop(positions):
+    """term_distance.rs:48-54: the max over consecutive lists (tuple_windows), u32::MAX with fewer than 2"""
+    pairs = [min_slop_two_positions(a, b) for a, b in zip(positions, positions[1:])]
+    return max(pairs) if pairs else U32_MAX
+
+
+def score_slop(slop):
+    return 1.0 / (float(slop) + 1.0)
+
+
+class Page:
+    """One ranking webpage: `signals` {SignalEnum name: (value, score)}, `score` (unboosted), `boost`, `key` the caller's id."""
+
+    def __init__(self, key, signals, score, boost):
+        self.key, self.signals, self.score, self.boost = key, dict(signals), float(score), float(boost)
+
+    def total(self):
+        return self.boost * self.score
+
+
+def pages_from_webpages(wp, q, docs, n, initial_totals):
+    """The pages of query q from ranking_webpages' result `wp` (its op names are the signals), the initial totals
+    (the top-k entry point's f64 totals, WebpagePointer.score.total) and the documents as keys.  MinTitleSlop / MinCleanBodySlop
+    are not signals yet: recall_stage computes them from min_slop."""
+    out = []
+    for i in range(n):
+        sig = {name: (float(wp.values[q, i, o]), float(wp.scores[q, i, o])) for o, name in enumerate(wp.names)}
+        p = Page(int(docs[i]), sig, initial_totals[i], wp.boosts[q, i])
+        p.min_slop = (int(wp.min_slop[q, i, 0]), int(wp.min_slop[q, i, 1]))
+        out.append(p)
+    return out
+
+
+def update_scores(pages, coefficients):
+    """FullRankingStage::update_scores: per page, fold from 0.0 over its present signals in SignalEnum order of
+    acc + score * coefficient -- sequential over the signals, vectorised over the pages, two roundings per step (no FMA)."""
+    if not pages:
+        return
+    acc = np.zeros(len(pages))
+    for name in SIGNAL_ENUM:
+        have = np.array([name in p.signals for p in pages])
+        if not have.any():
+            continue
+        sc = np.array([p.signals[name][1] if name in p.signals else 0.0 for p in pages])
+        prod = sc * np.float64(coefficients.get(name, 0.0))
+        acc = np.where(have, acc + prod, acc)
+    for p, a in zip(pages, acc):
+        p.score = float(a)
+
+
+def rank(pages):
+    """sort_by(b.score().partial_cmp(&a.score())): stable, descending boost * score"""
+    pages.sort(key=lambda p: -p.total())
+
+
+def _stage(pages, coefficients, compute):
+    compute(pages)
+    update_scores(pages, coefficients)
+    rank(pages)
+
+
+def recall_stage(pages, coefficients, inbound):
+    """RankingPipeline::recall_stage without LambdaMART: TitleDistanceScorer, BodyDistanceScorer, the two embedding stages (no
+    dual encoder: they insert nothing, embedding.rs:122-125, but still re-sum and rank), InboundScorer with `inbound`
+    {page key: score} (e.g. Webgraph.inbound_similarity), then the InboundSimilarity modifier.  Pages carry `min_slop`
+    (Title, CleanBody).  Returns the pages in their final order."""
+    pages = list(pages)
+    coefficients = dict(coefficients)
+
+    def distance(field, name):
+        def compute(ps):
+            for p in ps:
+                v = float(p.min_slop[field])
+                p.signals[name] = (v, score_slop(v))
+        return compute
+
+    _stage(pages, coefficients, distance(0, "MinTitleSlop"))
+    _stage(pages, coefficients, distance(1, "MinCleanBodySlop"))
+    _stage(pages, coefficients, lambda ps: None)   # TitleEmbeddings
+    _stage(pages, coefficients, lambda ps: None)   # KeywordEmbeddings
+
+    def inbound_scorer(ps):
+        for p in ps:
+            s = float(inbound[p.key])
+            p.signals["InboundSimilarity"] = (s, s)
+    _stage(pages, coefficients, inbound_scorer)
+    for p in pages:   # modifiers::InboundSimilarity: boost *= value + 8; no re-sum
+        v = p.signals["InboundSimilarity"][0] if "InboundSimilarity" in p.signals else 0.0
+        p.boost = p.boost * (v + INBOUND_SIMILARITY_SMOOTHING)
+    rank(pages)
+    return pages
