@@ -96,6 +96,11 @@ def declare(L):
         _lib_bm25.proto(L, f)
     except ImportError:
         pass
+    from . import _lib_lambdamart
+    try:
+        _lib_lambdamart.proto(L, f)
+    except AttributeError:   # a build of a subset of the sources (the CPU emulator library of the BM25 / HyperBall tests)
+        pass
     return L
 
 

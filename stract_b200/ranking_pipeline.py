@@ -5,7 +5,9 @@ A page is (signals, score, boost): `signals` maps a SignalEnum name to (value, s
 as its score and SignalComputer::boosts as its boost (recall.rs:198-217).  Each stage computes, then `update_scores` re-sums
 sum(score * coefficient) over the present signals in SignalEnum order (scorers/mod.rs:50-56), then `rank` sorts the pages
 stably by boost * score, descending.  The InboundSimilarity modifier multiplies the boost by value + 8 and re-ranks without
-re-summing.  LambdaMART, the embeddings themselves and the precision stage need models and are not mirrored."""
+re-summing.  With a model (stract_b200.lambdamart.LambdaMART, the reference's `lambda_model_path`) the LambdaMART stage follows:
+the top 20 pages are predicted on the device, re-summed and ranked, unless the query's offset is above 20.  The embeddings
+themselves and the precision stage need models the reference does not ship and are not mirrored."""
 import numpy as np
 
 from .bm25 import CORE_SIGNALS, NUMERIC_SIGNALS
@@ -111,14 +113,38 @@ def _stage(pages, coefficients, compute):
     rank(pages)
 
 
-def recall_stage(pages, coefficients, inbound):
-    """RankingPipeline::recall_stage without LambdaMART: TitleDistanceScorer, BodyDistanceScorer, the two embedding stages (no
-    dual encoder: they insert nothing, embedding.rs:122-125, but still re-sum and rank), InboundScorer with `inbound`
-    {page key: score} (e.g. Webgraph.inbound_similarity), then the InboundSimilarity modifier.  Pages carry `min_slop`
-    (Title, CleanBody).  Returns the pages in their final order."""
-    pages = list(pages)
-    coefficients = dict(coefficients)
+LAMBDAMART_TOP = 20   # Top::Limit(20), pipeline/scorers/lambdamart.rs:38-40
 
+
+def recall_stage(pages, coefficients, inbound, lambdamart=None, offset=0):
+    """RankingPipeline::recall_stage for one query: recall_stage_batch with one query."""
+    return recall_stage_batch([pages], coefficients, inbound, lambdamart, offset)[0]
+
+
+def recall_stage_batch(pages_per_query, coefficients, inbound, lambdamart=None, offset=0):
+    """RankingPipeline::recall_stage per query: TitleDistanceScorer, BodyDistanceScorer, the two embedding stages (no dual
+    encoder: they insert nothing, embedding.rs:122-125, but still re-sum and rank), InboundScorer with `inbound` {page key: score}
+    (e.g. Webgraph.inbound_similarity), the InboundSimilarity modifier, then with a `lambdamart` model the LambdaMART stage over
+    each query's top 20 (pipeline/mod.rs:136-162: skipped when `offset`, page * num_results, is above 20), predicted for every
+    query in one device call.  Pages carry `min_slop` (Title, CleanBody).  Returns each query's pages in their final order."""
+    coefficients = dict(coefficients)
+    out = [_recall_host_stages(list(pages), coefficients, inbound) for pages in pages_per_query]
+    if lambdamart is None or offset > LAMBDAMART_TOP:
+        return out
+    tops = [pages[:LAMBDAMART_TOP] for pages in out]
+    flat = [p for top in tops for p in top]
+    scores = lambdamart.predict(lambdamart.feature_rows(flat)) if flat else []
+    for p, s in zip(flat, scores):
+        p.signals["LambdaMart"] = (float(s), float(s))   # SignalCalculation::new_symmetrical
+    for pages, top in zip(out, tops):
+        update_scores(top, coefficients)
+        rank(top)
+        pages[:len(top)] = top
+    return out
+
+
+def _recall_host_stages(pages, coefficients, inbound):
+    """the stages before LambdaMART, in place on `pages`"""
     def distance(field, name):
         def compute(ps):
             for p in ps:
