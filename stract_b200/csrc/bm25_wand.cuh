@@ -161,6 +161,53 @@ __global__ void __launch_bounds__(WD_WARPS * 32) k_wand(const WandParams P) {
   unsigned long long guard = 64ull;
   for (uint32_t i = 0; i < n; i++) guard += 600ull * (sc[i].df + 256ull);   // a broken build fails instead of spinning
   bool watchdog = false;
+  // TopNComputer::push, then the collector's new threshold (the callback of both walks)
+  auto push = [&](float score, uint32_t doc) {
+    if (!(score > threshold)) return;
+    if (!(has_thr && score < thr)) {
+      if (count == tcap) {
+        w_sort_prefix_desc(khi, klo, count, P.cap, lane);
+        thr = unord_f32((uint32_t)(khi[top_n] >> 32)); has_thr = true; count = top_n;
+        __syncwarp();
+      }
+      if (lane == 0) { khi[count] = (uint64_t)ord_f32(score) << 32; klo[count] = ~doc; }
+      count++;
+      __syncwarp();
+    }
+    threshold = has_thr ? thr : -3.4028235e38f;
+  };
+
+  if (n == 1) {
+    // A one-clause query is not block_wand in the reference: the TermWeight runs block_wand_single_scorer
+    // (term_weight.rs:81-90, block_wand.rs:222-261).  It has no max_score cut-off, skips a block while its block max is
+    // below (not at) the threshold, and leaves a scored block with shallow_seek(last + 1), so the next block is not
+    // loaded: a VInt tail it has not loaded is bounded by max_score (block_segment_postings.rs:147-184), which is no
+    // bound on a large tf in a short document.  This walk restates it step by step.
+    WScorer& s = sc[0];
+    uint32_t* docs = WD_DOCS(0); uint32_t* tfs = WD_TFS(0);
+    uint32_t doc = docs[s.cur];
+    for (;;) {
+      if (guard-- == 0) { watchdog = true; break; }
+      bool done = false;
+      while (wd_block_max(P, s, docs, tfs, cache, lane) < threshold) {
+        if (s.last == TERMINATED) { done = true; break; }
+        doc = s.last + 1; wd_shallow_seek(P, s, doc); n_blocks++;
+      }
+      if (done) break;
+      doc = wd_seek(P, s, docs, tfs, scratch, doc, lane);
+      if (doc == TERMINATED) break;
+      bool ret = false;
+      for (;;) {
+        push(wd_score(s.weight, cache, P.S.fieldnorm[doc], tfs[s.cur]), doc); n_scored++;
+        if (doc == s.last) break;
+        doc = wd_advance(P, s, docs, tfs, scratch, lane);
+        if (doc == TERMINATED) { ret = true; break; }
+      }
+      if (ret) break;
+      doc += 1; wd_shallow_seek(P, s, doc);
+    }
+    n = 0;   // the block_wand loop below has nothing to do
+  }
 
 #define WD_RESTORE(ordinal)                                                              \
   do {                                                                                    \
@@ -218,19 +265,7 @@ __global__ void __launch_bounds__(WD_WARPS * 32) k_wand(const WandParams P) {
       for (uint32_t i = 0; i < plen; i++) { const uint32_t x = ord[i]; score = __fadd_rn(score, wd_score(sc[x].weight, cache, id, WD_TFS(x)[sc[x].cur])); }
     }
     n_scored++;
-    if (score > threshold) {   // callback: TopNComputer::push, then the collector's new threshold
-      if (!(has_thr && score < thr)) {
-        if (count == tcap) {
-          w_sort_prefix_desc(khi, klo, count, P.cap, lane);
-          thr = unord_f32((uint32_t)(khi[top_n] >> 32)); has_thr = true; count = top_n;
-          __syncwarp();
-        }
-        if (lane == 0) { khi[count] = (uint64_t)ord_f32(score) << 32; klo[count] = ~pivot; }
-        count++;
-        __syncwarp();
-      }
-      threshold = has_thr ? thr : -3.4028235e38f;
-    }
+    push(score, pivot);
     // advance_all_scorers_on_pivot
     for (uint32_t i = 0; i < plen; i++) { const uint32_t x = ord[i]; wd_advance(P, sc[x], WD_DOCS(x), WD_TFS(x), scratch, lane); }
     for (uint32_t i = 0; i != n;) { if (WD_DOC(ord[i]) == TERMINATED) { ord[i] = ord[n - 1]; n--; } else i++; }

@@ -10,15 +10,25 @@ from stract_b200.bm25 import MODE_AND, MODE_OR, NO_TERM, SegmentReader, SignalCo
 pytestmark = pytest.mark.gpu
 
 
-def build(term_docs, term_tfs, lens, record_option=1):
-    """The same index as an oracle Segment and as a device SegmentReader (library writer)."""
-    ids = bm25.fieldnorms_to_ids(lens)
+def total_num_tokens(ids):
+    """The sum of the fieldnorms of `ids` (u8 fieldnorm codes) without a per-doc wide temporary: np.bincount casts its
+    input to intp, so it runs over chunks (a 2^31-doc segment would otherwise take 17 GB)."""
+    counts = np.zeros(256, np.uint64)
+    for a in range(0, ids.size, 1 << 24):
+        counts += np.bincount(ids[a:a + (1 << 24)], minlength=256).astype(np.uint64)
+    return int((counts * bm25.fieldnorm_table().astype(np.uint64)).sum())
+
+
+def build(term_docs, term_tfs, lens, record_option=1, fieldnorm_ids=None):
+    """The same index as an oracle Segment and as a device SegmentReader (library writer).  `fieldnorm_ids` (u8 codes)
+    replaces `lens` when given."""
+    ids = bm25.fieldnorms_to_ids(lens) if fieldnorm_ids is None else np.ascontiguousarray(fieldnorm_ids, np.uint8)
     oseg = oracle.Segment(ids, record_option=record_option)
     for d, t in zip(term_docs, term_tfs):
         oseg.add_term(np.asarray(d, np.uint32), np.asarray(t, np.uint32))
     data, infos = bm25.encode_postings(term_docs, term_tfs, ids, oseg.avg_fieldnorm, record_option=record_option)
     assert np.array_equal(data, oseg.postings_bytes())
-    seg = SegmentReader(data, infos, ids, record_option=record_option, total_num_tokens=int(bm25.fieldnorm_table()[ids].astype(np.uint64).sum()))
+    seg = SegmentReader(data, infos, ids, record_option=record_option, total_num_tokens=total_num_tokens(ids))
     assert seg.average_fieldnorm == np.float32(oseg.avg_fieldnorm)
     return oseg, seg
 
@@ -238,11 +248,16 @@ def test_and3_unit_kernel_bit_exact(monkeypatch):
 
 
 def union_kernel_against_oracle(seed, max_doc, dfs, nq, ks, pad_every, sig_nq, sig_k):
+    """k_or3 against the oracle on a random index (see union_kernel_check)."""
+    (oseg, seg), rng = random_index(seed, max_doc, dfs)
+    union_kernel_check(oseg, seg, rng, nq, ks, pad_every, sig_nq, sig_k)
+
+
+def union_kernel_check(oseg, seg, rng, nq, ks, pad_every, sig_nq, sig_k, sig_cols=(4, 2, 0), sig_max_docs=(0,)):
     """k_or3 against the oracle: OR batches of 1/2/3/5/8 clauses (every `pad_every`-th query of 3+ clauses padded with
     NO_TERM) whose large queries are cut into doc-range items and merged, compared query by query with the exhaustive
-    union; and the signal combine with 4 / 2 / 0 columns."""
-    (oseg, seg), rng = random_index(seed, max_doc, dfs)
-    nt = len(dfs)
+    union; and the signal combine with `sig_cols` columns (k_or3, or k_topk_warp for a max_docs cut)."""
+    nt, max_doc = seg.n_terms, seg.max_doc
     for width in (1, 2, 3, 5, 8):
         terms = np.stack([rng.choice(nt, width, replace=False) for _ in range(nq)]).astype(np.uint32)
         if width >= 3:
@@ -257,18 +272,20 @@ def union_kernel_against_oracle(seed, max_doc, dfs, nq, ks, pad_every, sig_nq, s
                 assert m == len(od), (width, k, q, m, len(od))
                 assert np.array_equal(gd[q, :m], od) and np.array_equal(gs[q, :m], os_), (width, k, q)
     cache = bm25.compute_tf_cache(seg.average_fieldnorm)
-    for ncols in (4, 2, 0):
+    for ncols in sig_cols:
         cols = [rng.random(max_doc) for _ in range(ncols)]
         coeffs = [2.0, 0.02, 2.0, 0.001][:ncols]
         comp = SignalComputer(seg, SignalTable(cols) if ncols else None, coeffs, coeff_text=0.005)
         terms = np.stack([rng.choice(nt, 5, replace=False) for _ in range(sig_nq)]).astype(np.uint32)
         w = np.array([[bm25.StractBm25Weight.for_one_term(int(seg.doc_freq[t]), seg.max_doc, seg.average_fieldnorm).weight for t in row]
                       for row in terms], np.float32)
-        od, ot, on, _ = oseg.signal_topk_batch(terms, w, np.tile(cache, (sig_nq * 5, 1)), 1.2, 0.005, cols, coeffs, sig_k, threads=8)
-        gd, gt, gn = comp.top_docs_batch(terms, sig_k)
-        assert np.array_equal(gn, on), ncols
-        for q in range(sig_nq):
-            assert np.array_equal(gd[q, :gn[q]], od[q, :on[q]]) and np.array_equal(gt[q, :gn[q]], ot[q, :on[q]]), (ncols, q)
+        for max_docs in sig_max_docs:
+            od, ot, on, _ = oseg.signal_topk_batch(terms, w, np.tile(cache, (sig_nq * 5, 1)), 1.2, 0.005, cols, coeffs, sig_k,
+                                                   max_docs=max_docs, threads=8)
+            gd, gt, gn = comp.top_docs_batch(terms, sig_k, max_docs=max_docs)
+            assert np.array_equal(gn, on), (ncols, max_docs)
+            for q in range(sig_nq):
+                assert np.array_equal(gd[q, :gn[q]], od[q, :on[q]]) and np.array_equal(gt[q, :gn[q]], ot[q, :on[q]]), (ncols, max_docs, q)
 
 
 def test_or3_union_kernel_bit_exact():
