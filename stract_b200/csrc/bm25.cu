@@ -91,7 +91,7 @@ struct sb200_segment {
   sb200::DevBuf<uint8_t> pos_file;
   sb200::DevBuf<uint64_t> pos_data_off, pos_tail_off, pos_end_off, pos_count;   // per term
   sb200::DevBuf<uint32_t> pos_first, pos_nblk;                                   // per term
-  sb200::DevBuf<uint32_t> pos_b_off; sb200::DevBuf<uint8_t> pos_b_w;            // per positions block
+  sb200::DevBuf<uint64_t> pos_b_off; sb200::DevBuf<uint8_t> pos_b_w;            // per positions block
   sb200::DevBuf<uint64_t> pos_base;                                              // per posting block slot
   std::vector<uint64_t> h_pos_count;
   // scratch of the phrase path

@@ -33,7 +33,7 @@ struct PosView {
   const uint32_t* f32;                       // the positions file as words (+64 zero bytes)
   const uint64_t *data_off, *tail_off, *end_off, *count;   // per term
   const uint32_t *first, *nblk;              // per term: first block slot, bit-packed blocks
-  const uint32_t* b_off; const uint8_t* b_w; // per block: byte offset from data_off, bit width
+  const uint64_t* b_off; const uint8_t* b_w; // per block: byte offset from data_off (a term's blocks may pass 4 GiB), bit width
 };
 
 // 4 bytes of the file at any byte offset
@@ -497,7 +497,7 @@ __global__ void k_pos_dir(const uint8_t* __restrict__ file, const uint64_t* __re
                           const uint64_t* __restrict__ hdr, const uint32_t* __restrict__ nblk, const uint32_t* __restrict__ pfirst,
                           uint32_t n_terms, const uint8_t* __restrict__ postings, const uint64_t* __restrict__ t_data_off,
                           const uint32_t* __restrict__ t_df, const uint32_t* __restrict__ t_first,
-                          uint64_t* data_off, uint64_t* tail_off, uint64_t* end_off, uint64_t* count, uint32_t* b_off, uint8_t* b_w,
+                          uint64_t* data_off, uint64_t* tail_off, uint64_t* end_off, uint64_t* count, uint64_t* b_off, uint8_t* b_w,
                           uint64_t* pos_base, int* err) {
   const uint32_t t = (blockIdx.x * (uint32_t)blockDim.x + threadIdx.x) >> 5;
   if (t >= n_terms) return;
@@ -512,7 +512,7 @@ __global__ void k_pos_dir(const uint8_t* __restrict__ file, const uint64_t* __re
     if (w > 32) bad = true;
     const uint32_t size = w * 16u;
     const uint32_t incl = warp_scan_incl(size, lane);
-    if (j < nb) { b_off[first + j] = (uint32_t)(run + incl - size); b_w[first + j] = (uint8_t)w; }
+    if (j < nb) { b_off[first + j] = run + incl - size; b_w[first + j] = (uint8_t)w; }
     run += __shfl_sync(0xffffffffu, incl, 31);
   }
   const uint64_t tail = data + run;

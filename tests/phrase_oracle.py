@@ -176,7 +176,9 @@ def intersection_exists_with_slop(left, right, slop):
 
 
 def intersection_count_with_carrying_slop(left, left_slops, right, max_slop, update_left):
-    """returns (count, new left, new left_slops); slops are u8 (`as u8` truncates), an empty left_slops means 0 so far"""
+    """returns (count, new left, new left_slops); slops are u8 (`as u8` truncates), an empty left_slops means 0 so far.
+    `slop_so_far as u32 + abs_diff` is a u32 add that wraps in the reference's release build (phrase_scorer.rs:270,297,317,
+    327): a slop so far of s >= 1 and two positions at least 2^32 - s apart give a distance below s, which matches."""
     if not left or not right:
         return 0, ([] if update_left else left), ([] if update_left else left_slops)
     pb, sb = [], []
@@ -194,7 +196,7 @@ def intersection_count_with_carrying_slop(left, left_slops, right, max_slop, upd
         lv = left[i]
         sso = left_slops[i] if i < len(left_slops) else 0
         rv = right[j]
-        dist = sso + abs(lv - rv)
+        dist = (sso + abs(lv - rv)) & 0xFFFFFFFF
         if dist <= max_slop:
             if lv < rv:
                 smaller, larger, si, sp = lv, rv, i, left
@@ -207,7 +209,7 @@ def intersection_count_with_carrying_slop(left, left_slops, right, max_slop, upd
                 if nv > larger:
                     break
                 si += 1
-                new_slop = sso + abs(nv - larger)
+                new_slop = (sso + abs(nv - larger)) & 0xFFFFFFFF
                 add(new_slop, nv)
             add(new_slop, larger)
             count += 1; i += 1; j += 1
@@ -220,14 +222,14 @@ def intersection_count_with_carrying_slop(left, left_slops, right, max_slop, upd
                 lv = left[-1]
                 s0 = left_slops[-1] if left_slops else 0
                 for r in right[j:]:
-                    ns = abs(lv - r) + s0
+                    ns = (abs(lv - r) + s0) & 0xFFFFFFFF
                     if ns <= max_slop:
                         add(ns, r)
             else:
                 rv = right[-1]
                 for li in range(i, len(left)):
                     s0 = left_slops[li] if li < len(left_slops) else 0
-                    ns = abs(left[li] - rv) + s0
+                    ns = (abs(left[li] - rv) + s0) & 0xFFFFFFFF
                     if ns <= max_slop:
                         add(ns, left[li])
             break

@@ -289,3 +289,232 @@ def parse_positions(data, off, ln):
             p += 1; m += 1
         p += 1; lens.append(m)
     return widths, lens
+
+
+# ---- positional fixtures: phrases, optic patterns and term distances at wide positions ------------------------------------
+TOP = 0xFFFFFFFF
+
+
+def _anchor_streams(rng):
+    """The anchor's postings as position arrays: one full positions block per width in PW (one delta of that width, 127
+    small ones, split into ~13 postings that never straddle a block), a block of width 32 whose postings all start at or
+    above 2^31, then a VInt tail whose deltas take 1 to 5 bytes"""
+    streams = []
+    for w in PW:
+        if w == 0:      # every delta 0: 128 postings of tf 1 at position 0
+            streams += [np.zeros(1, np.int64)] * 128
+            continue
+        dl = rng.integers(1, min(1 << w, 8), 128, dtype=np.int64)
+        dl[int(rng.integers(0, 128))] = _wide(rng, w, (1 << 31) - 1)
+        streams += np.split(dl, np.sort(rng.choice(np.arange(1, 128), 12, replace=False)))
+    dl = rng.integers(1, 8, 128, dtype=np.int64)
+    cuts = np.arange(0, 128, 16)
+    dl[cuts] = (1 << 31) + rng.integers(0, 1 << 29, cuts.size)      # 8 postings of 16 positions from 2^31 up
+    streams += np.split(dl, cuts[1:])
+    for b in (1, 2, 3, 4, 5):   # the tail: each wide value opens a posting of its own
+        lo = 1 << (7 * (b - 1)) if b > 1 else 1
+        streams.append(np.array([int(rng.integers(lo, min((1 << (7 * b)) - 1, (1 << 31) - 1) + 1))] + list(rng.integers(1, 8, 2))))
+    pos = [np.cumsum(s) for s in streams]
+    assert all(int(p[-1]) < 1 << 32 for p in pos) and sum(p.size for p in pos) % 128 != 0
+    return [p.astype(np.uint32) for p in pos]
+
+
+def _spread_docs(rng, n, max_doc):
+    """n ascending doc ids over [0, max_doc): a dense run, a jump of about max_doc / 2 inside the first block, random
+    docs above it, and max_doc - 1 last"""
+    a = n // 3
+    dense = np.arange(a, dtype=np.int64) * 3
+    rest = np.sort(rng.choice(np.arange(max_doc // 2, max_doc - 1, dtype=np.int64), n - a - 1, replace=False))
+    return np.concatenate([dense, rest, [max_doc - 1]]).astype(np.uint32)
+
+
+def _partner(rng, docs, pos, keep, shift, frac=1.0):
+    """a term on the anchor's documents `keep` (indices), at the anchor's positions + shift (an int or a per-position
+    array drawer), on a fraction of the positions (at least one)"""
+    d, p = [], []
+    for i in keep:
+        x = pos[i].astype(np.int64)
+        if frac < 1.0:
+            x = x[np.sort(rng.choice(x.size, max(1, int(x.size * frac)), replace=False))]
+        s = shift(x.size) if callable(shift) else shift
+        y = np.unique(x + s)
+        d.append(docs[i]); p.append(y.astype(np.uint32))
+    return {"docs": np.array(d, np.uint32), "positions": p}
+
+
+def positional_range_index(seed, max_doc):
+    """A record-option-2 index over [0, max_doc) given as per-document positions (the form of
+    phrase_fixtures.make_segment).  Term roles (fx["roles"]):
+      anchor     one positions block per delta width in PW and one of width 32 (positions from 2^31 up), a VInt tail with
+                 1- to 5-byte deltas; its doc ids take wide doc deltas and end at max_doc - 1
+      plus1/2    the anchor's positions + 1 / + 2 on a subset of its postings: slop-0 phrases match at wide positions
+      near1..3   the anchor's positions + 1..3 (random per position): slop 1..3
+      df128 .. df257, vint   the anchor's positions + 1 on 128, 129, 256, 257 and 40 (VInt tail only) postings
+      wrap_a/b/c on documents where the anchor sits at position 0: wrap_a at 0, wrap_b at 4, wrap_c at 2^32 - 1.  The
+                 phrase (wrap_a, wrap_b, wrap_c) with offsets (0, 1, 2) and slop >= 3 carries slop 3 from the first pair
+                 into `3 + abs_diff(2, 2^32 - 1)`, which wraps to 0 in u32: it matches only because the sum wraps
+      big_a/b    one posting of tf 2^16 + 1 (among 127 others in a full block) and the same positions + 1: a verify pass
+                 over global scratch
+    `counted` = (docs, token counts) of the documents with positions (token_counts makes the dense column): it puts
+    num_tokens - 1 on the anchor's last position for its postings above 2^30 (end anchors at wide positions) and above
+    every position elsewhere.  Memory stays sparse up to max_doc = 2^31 - 2."""
+    from stract_b200.bm25 import fieldnorm_table
+    rng = np.random.default_rng(seed)
+    apos = _anchor_streams(rng)
+    adocs = _spread_docs(rng, len(apos), max_doc)
+    terms, roles = [{"docs": adocs, "positions": apos}], {"anchor": 0}
+
+    def add(name, t):
+        roles[name] = len(terms); terms.append(t)
+
+    na = len(apos)
+    sub = lambda n: np.sort(rng.choice(na, n, replace=False))
+    add("plus1", _partner(rng, adocs, apos, sub(int(na * 0.7)), 1, 0.8))
+    add("plus2", _partner(rng, adocs, apos, sub(int(na * 0.6)), 2, 0.8))
+    for s in (1, 2, 3):
+        add(f"near{s}", _partner(rng, adocs, apos, sub(int(na * 0.5)), lambda n, s=s: rng.integers(1, s + 1, n), 0.7))
+    for df in (128, 129, 256, 257, 40):
+        add("vint" if df < 128 else f"df{df}", _partner(rng, adocs, apos, sub(df), 1, 0.8))
+    zero = [i for i in range(na) if apos[i].size == 1 and apos[i][0] == 0]
+    wd = np.sort(rng.choice(zero, 12, replace=False))
+    one = lambda idx, p: {"docs": adocs[idx], "positions": [np.array([p], np.uint32)] * len(idx)}
+    add("wrap_a", one(wd[:6], 0))
+    add("wrap_b", one(wd[:8], 4))
+    add("wrap_c", one(wd[1:12], TOP))
+    # tf 2^16 + 1: the 200th posting of a 300-posting term over the anchor's doc range, and the same positions + 1
+    bd = np.sort(rng.choice(max_doc, 300, replace=False)).astype(np.uint32)
+    bp = [np.sort(rng.choice(1 << 20, int(rng.integers(1, 4)), replace=False)).astype(np.uint32) for _ in bd]
+    bp[200] = np.sort(rng.choice(1 << 24, TF16 + 1, replace=False)).astype(np.uint32)
+    add("big_a", {"docs": bd, "positions": bp})
+    add("big_b", {"docs": bd[195:205], "positions": [p + 1 for p in bp[195:205]]})
+    ids = np.empty(max_doc, np.uint8)
+    for a in range(0, max_doc, 1 << 26):
+        ids[a:a + (1 << 26)] = rng.integers(0, 256, min(1 << 26, max_doc - a), dtype=np.uint8)
+    table = fieldnorm_table().astype(np.uint64)
+    total = sum(int(np.bincount(ids[a:a + (1 << 26)], minlength=256) @ table) for a in range(0, max_doc, 1 << 26))
+    last = {}
+    for t in terms:
+        for d, p in zip(t["docs"], t["positions"]):
+            last[int(d)] = max(last.get(int(d), 0), int(p[-1]) + 1)
+    posted = np.array(sorted(last), np.int64)
+    cvals = np.array([last[int(d)] for d in posted], np.uint64) + rng.integers(0, 3, posted.size).astype(np.uint64)
+    wide = [i for i in range(na) if int(apos[i][-1]) >= 1 << 30]
+    cvals[np.searchsorted(posted, adocs[wide])] = [last[int(d)] for d in adocs[wide]]
+    return {"fieldnorm_ids": ids, "terms": terms, "total_num_tokens": total, "roles": roles, "counted": (posted, cvals),
+            "max_doc": max_doc, "end_anchored": adocs[wide]}
+
+
+def token_counts(fx):
+    """the dense token-count column of a positional_range_index (one u64 per document; 0 for documents without positions)"""
+    c = np.zeros(fx["max_doc"], np.uint64)
+    c[fx["counted"][0]] = fx["counted"][1]
+    return c
+
+
+def token_count(fx, d):
+    posted, cvals = fx["counted"]
+    i = int(np.searchsorted(posted, d))
+    return int(cvals[i]) if i < posted.size and posted[i] == d else 0
+
+
+def positional_self_check(fx):
+    """every target of positional_range_index was produced: anchor block widths PW + 32 and 1- to 5-byte tail deltas in the
+    `.pos` bytes, doc ids up to max_doc - 1 and wide doc deltas in the postings, the doc_freqs, slop-0 matches at positions
+    >= 2^31, the u32 wrap (a match the unwrapped sum would reject), the tf 2^16 + 1 posting, and end-anchored documents
+    whose last position is >= 2^30.  Returns the anchor's widths and tail lengths and its largest doc-delta width."""
+    import phrase_oracle as O
+    from stract_b200.bm25 import encode_positions, encode_postings
+    terms, roles = fx["terms"], fx["roles"]
+    tfs = [np.array([p.size for p in t["positions"]], np.uint32) for t in terms]
+    off = np.concatenate([[0], np.cumsum([t["docs"].size for t in terms])])
+    pos, po, pl = encode_positions(np.concatenate([p for t in terms for p in t["positions"]]), np.concatenate(tfs), off)
+    widths, lens = parse_positions(pos, po[0], pl[0])
+    assert set(widths) == set(PW) | {32} and set(lens) >= {1, 2, 3, 4, 5}, (sorted(set(widths)), sorted(set(lens)))
+    data, infos = encode_postings([t["docs"] for t in terms], tfs, fx["fieldnorm_ids"], 1.0, record_option=2)
+    a = parse_term(data, infos[0].postings_off, infos[0].postings_len, infos[0].doc_freq, 2)
+    assert max(a["db"]) >= (20 if fx["max_doc"] > 1 << 22 else 9), a["db"]
+    assert int(max(t["docs"][-1] for t in terms)) == fx["max_doc"] - 1
+    dfs = {t["docs"].size for t in terms}
+    assert {128, 129, 256, 257} <= dfs and min(dfs) < 128
+    assert max(int(t.max()) for t in tfs) == TF16 + 1
+    cache = O.tf_cache(np.float32(1.0), np.arange(256))
+    idx = {"fieldnorm_ids": fx["fieldnorm_ids"], "terms": terms}
+    hits = O.phrase_search(idx, [roles["anchor"], roles["plus1"]], [0, 1], 0, True, np.float32(1.0), cache)
+    anchor = terms[roles["anchor"]]
+    assert any(int(anchor["positions"][int(np.searchsorted(anchor["docs"], d))][-1]) >= 1 << 31 for _, d in hits)
+    wq = [roles["wrap_a"], roles["wrap_b"], roles["wrap_c"]]
+    wh = O.phrase_search(idx, wq, [0, 1, 2], 3, True, np.float32(1.0), cache)
+    assert wh and all(int(x) == TOP for d in (h[1] for h in wh)
+                      for x in terms[wq[2]]["positions"][int(np.searchsorted(terms[wq[2]]["docs"], d))]), "the wrap case"
+    ea = fx["end_anchored"]
+    assert ea.size and all(token_count(fx, d) - 1 >= 1 << 30 for d in ea)
+    return widths, lens, max(a["db"])
+
+
+HUGE_TF = 1 << 28     # positions per huge posting: 1 GiB of 32-bit deltas each
+
+
+def huge_positions_term(seed, n_huge=5, late_tfs=(40, 90, 126, 3, 60, 5), max_doc=64):
+    """One term whose positions pass 4 GiB of bit-packed data, written straight to bytes.  At bit width 32 a BitPacker4x
+    block is its 128 values as little-endian u32 in order, so the `.pos` data of the n_huge postings of tf HUGE_TF is the
+    delta array itself: small deltas and one value with bit 31 set per block.  After them come `late_tfs` small postings
+    with ordinary deltas, whose full blocks (real widths) start past byte 4 GiB of the term's data; the rest is VInt tail.
+    df < 128: the postings are all VInt tail, so no skip entry sums a tf.
+
+    Term 0 is that term (docs 0 .. n_huge-1 huge, then the late docs); term 1 is a partner on the late docs only, at the
+    late positions + 1 (a subset, and one doc at + 3), so a phrase (0, 1) has only late candidates.  Positions of term 1
+    come first in the file, then pad bytes, then term 0, so that term 0's block data starts 4-byte aligned in memory.
+    Returns a dict: pos (u8 file), po / pl (ranges), deltas (u32 view of the huge region), late (the late postings'
+    deltas), index (the oracle index of the late postings of term 0 and all of term 1), docs / tfs per term, ids, total,
+    data_off (byte offset of term 0's block data in the file), late_off (position offset of the first late posting)."""
+    import phrase_oracle as O
+    rng = np.random.default_rng(seed)
+    late_pos = []
+    for tf in late_tfs:
+        d = rng.integers(1, 40, tf, dtype=np.int64)
+        if tf > 50:
+            d[tf // 2] = (1 << 31) + int(rng.integers(0, 1 << 20))   # late positions at and above 2^31
+        late_pos.append(np.cumsum(d).astype(np.uint32))
+    late = np.concatenate([np.diff(p, prepend=np.uint32(0)).astype(np.uint32) for p in late_pos])
+    hb = n_huge * HUGE_TF // 128
+    lb = late.size // 128
+    late_blocks = [O._bitpack4x(late[b * 128:(b + 1) * 128]) for b in range(lb)]
+    head = bytes(O._vint(hb + lb)) + bytes([32]) * hb + bytes(w for w, _ in late_blocks)
+    tail = b"".join(p for _, p in late_blocks) + b"".join(bytes(O._vint(int(x))) for x in late[lb * 128:])
+    # term 1: the partner's positions, serialized by the oracle writer
+    ldocs = np.arange(n_huge, n_huge + len(late_tfs), dtype=np.uint32)
+    p1, d1 = [], []
+    for i, p in enumerate(late_pos):
+        if i == 1:
+            continue                                              # a late doc without the partner
+        x = p[np.sort(rng.choice(p.size, max(1, p.size // 2), replace=False))].astype(np.int64)
+        p1.append((x + (3 if i == 3 else 1)).astype(np.uint32)); d1.append(ldocs[i])
+    t1 = O.serialize_positions(np.concatenate([np.diff(p, prepend=np.uint32(0)) for p in p1]).astype(np.uint32))
+    pad = (-(len(t1) + len(head))) % 4
+    data_off = len(t1) + pad + len(head)
+    nbytes = data_off + hb * 512 + len(tail)
+    pos = np.zeros(nbytes, np.uint8)
+    pos[:len(t1)] = np.frombuffer(t1, np.uint8)
+    pos[len(t1) + pad:data_off] = np.frombuffer(head, np.uint8)
+    deltas = pos[data_off:data_off + hb * 512].view(np.uint32)
+    step = 1 << 24
+    for a in range(0, deltas.size, step):
+        deltas[a:a + step] = rng.integers(0, 8, min(step, deltas.size - a), dtype=np.uint32)
+    blk = deltas.reshape(hb, 128)
+    blk[np.arange(hb), rng.integers(0, 128, hb)] = rng.integers(1 << 31, 1 << 32, hb, dtype=np.uint64).astype(np.uint32)
+    pos[data_off + hb * 512:] = np.frombuffer(tail, np.uint8)
+    po = np.array([len(t1) + pad, 0], np.uint64)
+    pl = np.array([nbytes - len(t1) - pad, len(t1)], np.uint64)
+    docs = [np.concatenate([np.arange(n_huge, dtype=np.uint32), ldocs]), np.array(d1, np.uint32)]
+    tfs = [np.array([HUGE_TF] * n_huge + list(late_tfs), np.uint32), np.array([p.size for p in p1], np.uint32)]
+    ids = rng.integers(0, 256, max_doc).astype(np.uint8)
+    from stract_b200.bm25 import fieldnorm_table
+    total = int(fieldnorm_table()[ids].astype(np.uint64).sum())
+    index = {"fieldnorm_ids": ids, "total_num_tokens": total,
+             "terms": [{"docs": ldocs, "positions": late_pos}, {"docs": docs[1], "positions": p1}]}
+    late_off = n_huge * HUGE_TF
+    # self-check: the late blocks start past 4 GiB of the term's data, the bytes parse back, a phrase matches there
+    assert data_off % 4 == 0 and late_off * 4 > 1 << 32 and lb >= 2
+    assert O.serialize_positions(late) == bytes(O._vint(lb)) + head[-lb:] + tail, "the late part as the writer has it"
+    return {"pos": pos, "po": po, "pl": pl, "deltas": deltas, "late": late, "index": index, "docs": docs, "tfs": tfs, "ids": ids,
+            "total": total, "data_off": data_off, "late_off": late_off, "n_huge": n_huge}

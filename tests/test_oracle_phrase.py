@@ -180,3 +180,27 @@ def test_library_writer_equals_oracle_writer():
         absolute = np.cumsum(deltas.astype(np.uint64)).astype(np.uint32)
         d, _, _ = encode_positions(absolute, [deltas.size], [0, 1])
         assert d.tobytes() == O.serialize_positions(deltas)
+
+
+def test_carrying_slop_distance_wraps_in_u32():
+    """`slop_so_far as u32 + abs_diff` wraps in the reference's release build (phrase_scorer.rs:270,317,327): a left
+    position carrying slop 1 and a right position 2^32 - 1 away are at distance 0.  Hand-made lists for the main loop and
+    both finish-rest branches, then a three-term phrase over one document, in the Python and the native oracle."""
+    top = 0xFFFFFFFF
+    c, left, slops = O.intersection_count_with_carrying_slop([0], [], [1], 1, True)
+    assert (c, left, slops) == (1, [0, 1], [1, 1])
+    assert O.intersection_count_with_carrying_slop(left, slops, [top], 1, False)[0] == 1        # main loop
+    assert O.intersection_count_with_carrying_slop([0], [1], [5, top], 1, True) == (0, [top], [0])      # left exhausted
+    assert O.intersection_count_with_carrying_slop([5, top], [1, 1], [0], 1, True) == (0, [top], [0])   # right exhausted
+    assert O.intersection_count_with_carrying_slop([0], [1], [top - 1], 1, True) == (0, [], [])         # no wrap: 2^32 - 1
+    from phrase_fixtures import index_to_csr, native_batch
+    one = lambda p: {"docs": np.array([0], np.uint32), "positions": [np.array([p], np.uint32)]}
+    idx = {"fieldnorm_ids": np.array([3], np.uint8), "terms": [one(0), one(1), one(top)], "total_num_tokens": 3}
+    cache = O.tf_cache(np.float32(3.0), np.arange(256))
+    w = O.bm25_weight_for_terms([1, 1, 1], 1)
+    for slop, n in ((1, 1), (300, 1), (0, 0)):
+        hits = O.phrase_search(idx, [0, 1, 2], [0, 0, 0], slop, True, w, cache)
+        assert len(hits) == n, slop
+        d, s, c = native_batch(index_to_csr(idx), np.array([[0, 1, 2]], np.uint32), np.zeros((1, 3), np.uint32),
+                               np.array([slop], np.uint32), [w], cache, True, 4, threads=1)
+        assert int(c[0]) == n and (not n or (d[0, 0] == 0 and s[0, 0].view(np.uint32) == hits[0][0].view(np.uint32))), slop
