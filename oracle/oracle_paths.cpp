@@ -31,7 +31,10 @@ static Csr build(uint32_t n, const uint32_t* from, const uint32_t* to, uint64_t 
 static void dijkstra_multi(const Csr& g, const uint32_t* sources, uint32_t n_sources, int max_dist /* < 0: None */, uint8_t* dist) {
   typedef std::pair<uint8_t, uint32_t> St;
   std::priority_queue<St, std::vector<St>, std::greater<St>> q;   // BinaryHeap of Reverse((cost, node))
-  for (uint32_t i = 0; i < n_sources; i++) { q.push({0, sources[i]}); dist[sources[i]] = 0; }
+  for (uint32_t i = 0; i < n_sources; i++) {
+    if (sources[i] == 0xFFFFFFFFu) continue;   // an id that is not a node reaches nothing (the device skips it too)
+    q.push({0, sources[i]}); dist[sources[i]] = 0;
+  }
   while (!q.empty()) {
     const St st = q.top(); q.pop();
     const uint8_t cost = st.first; const uint32_t v = st.second;

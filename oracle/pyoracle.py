@@ -279,7 +279,8 @@ def graph_distances(n, from_rank, to_rank, sources, groups=None, max_dist=None, 
 
 
 def approx_harmonic(n, from_rank, to_rank, sources, max_dist=7, num_nodes=None):
-    """ApproxHarmonic::build for a fixed sample: (f32 sums in source order, f64 sums of the same f32 terms), 0 = not reached."""
+    """ApproxHarmonic::build for a fixed sample: (f32 sums in source order, f64 sums of the same f32 terms), 0 = not reached.
+    A source rank 0xFFFFFFFF (an id that is not a node) counts in the sample size and reaches nothing."""
     fr = np.ascontiguousarray(from_rank, np.uint32); tr = np.ascontiguousarray(to_rank, np.uint32)
     src = np.ascontiguousarray(sources, np.uint32)
     o32 = np.zeros(n, np.float32); o64 = np.zeros(n, np.float64)
