@@ -6,4 +6,4 @@ import this package.  It is a ctypes binding over oracle/liboracle.so (built by 
 from .pyoracle import *  # noqa: F401,F403
 from .pyoracle_p2 import (Segment, Cursor, fieldnorm_to_id, id_to_fieldnorm, fieldnorms_to_ids,  # noqa: F401,E402
                          fieldnorm_table, tv_bm25_weight, stract_bm25_weight, term_info_store_write,
-                         term_info_store_get, bitpack, extract_bits, multi_signal_topk, numeric_scores)
+                         term_info_store_get, bitpack, extract_bits, multi_signal_topk, numeric_scores, topn_f64)

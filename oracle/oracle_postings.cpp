@@ -390,12 +390,26 @@ struct TermScorer {  // term_scorer.rs
 };
 
 // ---------------------------------------------------------------- TopNComputer ---------------
+// Order keys.  f32 BM25 scores are finite and >= 0: plain `>`.  f64 recall totals may be negative, -0.0, +-inf or NaN:
+// f64::total_cmp over the bits (the reference's ScoredDoc::cmp, collector/top_docs.rs:229-233), -0.0 below +0.0, with every
+// NaN first made the one negative quiet NaN 0xFFF8000000000000, so all NaN totals tie below -inf whatever sign their
+// computation left (DESIGN §5).  The device's ord_f64 (bm25.cu) is the same map.
+static inline float order_key(float f) { return f; }
+static inline uint64_t order_key(double f) {
+  uint64_t b; memcpy(&b, &f, 8);
+  if (f != f) b = 0xFFF8000000000000ull;
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
 template <class S>
 struct TopN {  // top_score_collector.rs:440-564 with ComparableDoc order (score desc, doc asc)
   struct E { S feature; uint32_t doc; };
   std::vector<E> buf; size_t top_n, cap; bool has_thr = false; S thr{};
   explicit TopN(size_t n) : top_n(n), cap(std::max<size_t>(n, 1) * 2) { buf.reserve(cap); }
-  static bool before(const E& a, const E& b) { if (a.feature != b.feature) return a.feature > b.feature; return a.doc < b.doc; }
+  static bool before(const E& a, const E& b) {
+    const auto ka = order_key(a.feature), kb = order_key(b.feature);
+    if (ka != kb) return ka > kb;
+    return a.doc < b.doc;
+  }
   S truncate() {
     std::nth_element(buf.begin(), buf.begin() + top_n, buf.end(), before);
     S med = buf[top_n].feature;
@@ -403,7 +417,7 @@ struct TopN {  // top_score_collector.rs:440-564 with ComparableDoc order (score
     return med;
   }
   void push(S f, uint32_t d) {
-    if (has_thr && f < thr) return;
+    if (has_thr && order_key(f) < order_key(thr)) return;
     if (buf.size() == cap) { thr = truncate(); has_thr = true; }
     buf.push_back({f, d});
   }
@@ -592,6 +606,16 @@ ORC_API uint32_t orc_bm25_topk(void* seg, const uint32_t* terms, const float* we
   if (mode == 0) return and_topk(s, terms, weights, caches, n_terms, k, docs, scores, scored);
   if (mode == 1) return or_topk(s, terms, weights, caches, n_terms, k, docs, scores, scored);
   return or_topk_exhaustive(s, terms, weights, caches, n_terms, k, docs, scores, scored);
+}
+
+// TopN<double> over a caller's (total, doc) list in the given push order, for hand-made lists of special values
+ORC_API uint32_t orc_topn_f64(const double* totals, const uint32_t* docs, uint32_t n, uint32_t k, uint32_t* out_docs, double* out_totals) {
+  if (k == 0) return 0;
+  TopN<double> top(k);
+  for (uint32_t i = 0; i < n; i++) top.push(totals[i], docs[i]);
+  auto v = top.into_sorted();
+  for (size_t i = 0; i < v.size(); i++) { out_docs[i] = v[i].doc; out_totals[i] = v[i].feature; }
+  return (uint32_t)v.size();
 }
 
 // Stract recall stage on one text field (path 2B): MainCollector over the Should-union of the query terms

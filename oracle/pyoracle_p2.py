@@ -45,6 +45,7 @@ def proto(L, f):
       _f64p, _u32p, _u64p)
     f("orc_multi_signal_topk", u32, u32, vp, vp, _f32p, _f32p, u32, _u8p, _u32p, _f32p, _f32p, vp, u32, _u32p, _u32p, _u32p, _u32p, _f64p,
       vp, u32, _u32p, _f64p, C.POINTER(u64))
+    f("orc_topn_f64", u32, _f64p, _u32p, u32, u32, _u32p, _f64p)
     f("orc_cursor_open", vp, vp, u32, f32, _f32p)
     f("orc_cursor_free", None, vp)
     for name in ("doc", "tf", "advance", "last_doc_in_block"):
@@ -224,6 +225,14 @@ def multi_signal_topk(segments, caches, k1s, coefs, slot_field, slot_term, slot_
                                 np.ascontiguousarray(o[:, 0]), np.ascontiguousarray(o[:, 1]), np.ascontiguousarray(o[:, 2]),
                                 np.ascontiguousarray(o[:, 3]), oc, C.cast(sarr, C.c_void_p), k, docs, totals, C.byref(sc))
     return docs[:n], totals[:n]
+
+
+def topn_f64(totals, docs, k):
+    """The oracle's TopN<double> over (total, doc) pairs pushed in the given order.  Returns (docs, totals)."""
+    t = np.ascontiguousarray(totals, np.float64); d = np.ascontiguousarray(docs, np.uint32)
+    od = np.zeros(max(k, 1), np.uint32); ot = np.zeros(max(k, 1), np.float64)
+    n = _L().orc_topn_f64(t, d, t.size, k, od, ot)
+    return od[:n], ot[:n]
 
 
 class Cursor:

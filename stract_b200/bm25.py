@@ -546,6 +546,27 @@ class TopDocs:
         return [(float(s[0, i]), int(d[0, i])) for i in range(int(n[0]))]
 
 
+def total_order_key(scores):
+    """int64 keys that order f64 scores (or f32 ones, widened exactly) as the device's top-k does: f64::total_cmp (collector/
+    top_docs.rs:229-233: -0.0 below +0.0, -inf / +inf at the ends) with every NaN first made the negative quiet NaN
+    0xFFF8000000000000, so NaNs tie below -inf (DESIGN §5).  A bigger key ranks first."""
+    x = np.array(scores, np.float64, ndmin=1)
+    b = x.view(np.int64)
+    b[np.isnan(x)] = np.int64(-0x0008000000000000)   # the bits 0xFFF8000000000000
+    return np.where(b < 0, b ^ np.int64(0x7FFFFFFFFFFFFFFF), b)
+
+
+def merge_fruits(parts, q, limit, offset=0):
+    """The per-segment top lists of query q merged (TopCollector::merge_fruits, top_collector.rs:109-129, and the recall
+    stage's BucketCollector, whose ScoredDoc::cmp is total_cmp): order (total_order_key desc, segment_ord asc, doc asc), the
+    first `offset` dropped.  parts = [(segment_ord, docs [nq,k], scores [nq,k], n [nq])].  Returns (segs, docs, scores)."""
+    segs = np.concatenate([np.full(int(n[q]), s_ord, np.uint32) for s_ord, _, _, n in parts])
+    docs = np.concatenate([d[q, :n[q]] for _, d, _, n in parts])
+    scs = np.concatenate([sc[q, :n[q]] for _, _, sc, n in parts])
+    order = np.lexsort((docs, segs, ~total_order_key(scs)))[offset:offset + limit]
+    return segs[order], docs[order], scs[order]
+
+
 class Searcher:
     """tantivy `Searcher` + `TopDocs` over several segments of one field.  The BM25 statistics are the index-wide ones
     (Bm25StatisticsProvider / Bm25Weight::for_terms, tantivy/src/query/bm25.rs:15-50,98-134: total_num_docs,
@@ -592,12 +613,9 @@ class Searcher:
         out_seg = np.zeros((nq, k), np.uint32); out_doc = np.zeros((nq, k), np.uint32)
         out_sc = np.zeros((nq, k), np.float32); out_n = np.zeros(nq, np.uint32)
         for q in range(nq):
-            segs = np.concatenate([np.full(int(n[q]), s_ord, np.uint32) for s_ord, _, _, n in parts])
-            docs = np.concatenate([d[q, :n[q]] for _, d, _, n in parts])
-            scs = np.concatenate([sc[q, :n[q]] for _, _, sc, n in parts])
-            order = np.lexsort((docs, segs, -scs.astype(np.float64)))[top_docs.offset:top_docs.offset + k]
-            m = order.size
-            out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = segs[order], docs[order], scs[order], m
+            sg, dc, sc_ = merge_fruits(parts, q, k, top_docs.offset)
+            m = dc.size
+            out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = sg, dc, sc_, m
         return out_seg, out_doc, out_sc, out_n
 
     def search_phrase_batch(self, top_docs, term_ords_per_segment, offsets=None, slop=None, scoring=True):
@@ -625,12 +643,9 @@ class Searcher:
         out_seg = np.zeros((nq, k), np.uint32); out_doc = np.zeros((nq, k), np.uint32)
         out_sc = np.zeros((nq, k), np.float32); out_n = np.zeros(nq, np.uint32)
         for q in range(nq):
-            segs = np.concatenate([np.full(int(n[q]), s_ord, np.uint32) for s_ord, _, _, n in parts])
-            docs = np.concatenate([d[q, :n[q]] for _, d, _, n in parts])
-            scs = np.concatenate([sc[q, :n[q]] for _, _, sc, n in parts])
-            order = np.lexsort((docs, segs, -scs.astype(np.float64)))[top_docs.offset:top_docs.offset + k]
-            m = order.size
-            out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = segs[order], docs[order], scs[order], m
+            sg, dc, sc_ = merge_fruits(parts, q, k, top_docs.offset)
+            m = dc.size
+            out_seg[q, :m], out_doc[q, :m], out_sc[q, :m], out_n[q] = sg, dc, sc_, m
         return out_seg, out_doc, out_sc, out_n
 
 
@@ -696,8 +711,9 @@ class SignalComputer:
 class SignalSearcher:
     """Path B over several segments: Stract's MultiBm25Weight::for_terms sums total_num_tokens / total_num_docs over the
     segment readers and takes doc_freq from the searcher (core/src/ranking/bm25.rs:52-92); every segment collects its top
-    k by `total` and the fruits are merged by (total desc, (segment_ord, doc) asc) like any tantivy top collector
-    (tweak_score_top_collector.rs -> TopCollector::merge_fruits, top_collector.rs:109-129)."""
+    k by `total` and the fruits are merged by (total desc, (segment_ord, doc) asc), the total ordered as the recall
+    collector orders it (MainCollector = TweakedScoreTopCollector: per-segment harvest and merge_fruits both go through
+    BucketCollector, whose ScoredDoc::cmp is f64::total_cmp) with the device's NaN rule -- see merge_fruits."""
 
     def __init__(self, computers):
         self.computers = list(computers)          # one SignalComputer per segment (same coefficients)
@@ -724,12 +740,9 @@ class SignalSearcher:
         out_seg = np.zeros((nq, k), np.uint32); out_doc = np.zeros((nq, k), np.uint32)
         out_t = np.zeros((nq, k), np.float64); out_n = np.zeros(nq, np.uint32)
         for q in range(nq):
-            segs = np.concatenate([np.full(int(n[q]), s_ord, np.uint32) for s_ord, _, _, n in parts])
-            docs = np.concatenate([d[q, :n[q]] for _, d, _, n in parts])
-            tot = np.concatenate([t[q, :n[q]] for _, _, t, n in parts])
-            order = np.lexsort((docs, segs, -tot))[:k]
-            m = order.size
-            out_seg[q, :m], out_doc[q, :m], out_t[q, :m], out_n[q] = segs[order], docs[order], tot[order], m
+            sg, dc, tt = merge_fruits(parts, q, k)
+            m = dc.size
+            out_seg[q, :m], out_doc[q, :m], out_t[q, :m], out_n[q] = sg, dc, tt, m
         return out_seg, out_doc, out_t, out_n
 
 

@@ -10,12 +10,26 @@ the host -- like the reference's, which runs it once per segment at harvest time
 documents.  What the GPU contributes is the candidate list: `harvest_top_k` feeds the collector the top-K documents by
 `total` and proves K was enough (see there).
 
+Order: documents pop by `f64::total_cmp` on the adjusted score, as `ScoredDoc::cmp` orders them (top_docs.rs:229-233), so
+-0.0 sits below +0.0, -inf below every number and a NaN ranks by its sign bit (a positive NaN above +inf, a negative one below
+-inf).  The reference's `update_best_doc` compares the re-adjusted score with `==`, which never holds for a NaN, so a NaN best
+document would loop there forever; this mirror compares the two scores' bits instead and so ranks a NaN by its bits and
+terminates.  The device's top-k hands every NaN total over as the negative NaN 0xFFF8000000000000 (DESIGN §5), which this
+order puts last.
+
 Tie note: the reference keeps the documents in a `min_max_heap::MinMaxHeap`; which of two documents with EQUAL adjusted
 score pops first is a property of that crate (not part of the reference tree).  This mirror pops the earlier-inserted one.
 """
 import heapq
+import struct
 
 import numpy as np
+
+
+def total_cmp_key(x):
+    """An int that orders f64 values as `f64::total_cmp` does (core::f64::total_cmp: flip the magnitude bits of negatives)."""
+    b = struct.unpack("<q", struct.pack("<d", float(x)))[0]
+    return b ^ 0x7FFFFFFFFFFFFFFF if b < 0 else b
 
 
 class CollectorConfig:
@@ -57,7 +71,7 @@ class BucketCollector:
         self.top_n = top_n
         self.config = config or CollectorConfig()
         self.buckets = {}
-        self._heap = []   # (-adjusted_score, insertion index, score, hashes, payload)
+        self._heap = []   # (-total_cmp_key(adjusted score), insertion index, adjusted score, score, hashes, payload)
         self._seq = 0
 
     def _adjusted(self, score, h):
@@ -68,7 +82,8 @@ class BucketCollector:
         return score * adjuster
 
     def insert(self, score, hashes, payload=None):
-        heapq.heappush(self._heap, (-self._adjusted(score, hashes), self._seq, float(score), hashes, payload))
+        adj = self._adjusted(score, hashes)
+        heapq.heappush(self._heap, (-total_cmp_key(adj), self._seq, adj, float(score), hashes, payload))
         self._seq += 1
 
     def _update_counts(self, h):
@@ -79,25 +94,25 @@ class BucketCollector:
         if len(self._heap) <= 1:
             return
         while self._heap:
-            neg, seq, score, h, payload = self._heap[0]
+            neg, seq, _adj, score, h, payload = self._heap[0]
             new = self._adjusted(score, h)
-            if new == -neg:
+            if total_cmp_key(new) == -neg:   # the same bits (the reference's `==` would never end on a NaN)
                 break
-            heapq.heapreplace(self._heap, (-new, seq, score, h, payload))
+            heapq.heapreplace(self._heap, (-total_cmp_key(new), seq, new, score, h, payload))
 
     def into_sorted_vec(self, de_rank_similar=True, with_adjusted=False):
         res, dups, table = [], [], SimhashTable()
         while self._heap:
-            neg, _seq, score, h, payload = heapq.heappop(self._heap)
+            _neg, _seq, adj, score, h, payload = heapq.heappop(self._heap)
             if h.simhash != 0 and de_rank_similar:
                 if table.contains(h.simhash):
-                    dups.append((payload, -neg))
+                    dups.append((payload, adj))
                     continue
                 table.insert(h.simhash)
             if de_rank_similar:
                 self._update_counts(h)
                 self._update_best_doc()
-            res.append((payload, -neg))
+            res.append((payload, adj))
             if len(res) == self.top_n:
                 break
         res.extend(dups[:max(self.top_n - len(res), 0)])

@@ -187,7 +187,13 @@ __global__ void k_build_directory(const uint8_t* __restrict__ postings, const sb
 // ------------------------------------------------------------------ device helpers ---------------
 __device__ __forceinline__ uint32_t ord_f32(float f) { const uint32_t b = __float_as_uint(f); return (b & 0x80000000u) ? ~b : (b | 0x80000000u); }
 __device__ __forceinline__ float unord_f32(uint32_t o) { return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o); }
-__device__ __forceinline__ uint64_t ord_f64(double f) { const uint64_t b = (uint64_t)__double_as_longlong(f); return (b >> 63) ? ~b : (b | 0x8000000000000000ull); }
+// f64 totals order by f64::total_cmp (collector/top_docs.rs:229-233: -0.0 below +0.0, +-inf at the ends), except that every
+// NaN is first made the negative quiet NaN 0xFFF8000000000000: a NaN total ranks below -inf whatever sign and payload it
+// carries (a NaN column keeps its own through the combine), never meets the (0, 0) padding key, and unord_f64 returns that NaN
+__device__ __forceinline__ uint64_t ord_f64(double f) {
+  const uint64_t b = f != f ? 0xFFF8000000000000ull : (uint64_t)__double_as_longlong(f);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
 __device__ __forceinline__ double unord_f64(uint64_t o) { return __longlong_as_double((long long)((o >> 63) ? (o & 0x7FFFFFFFFFFFFFFFull) : ~o)); }
 
 // first index in the sorted 128-entry block with value >= x (branchless, block_search.rs:23-34)

@@ -134,5 +134,6 @@ def optic_topk(candidates, k, rules=(), exclude=None, require=None):
         if rules:
             t = float(np.float64(t) * np.float64(boost_factor(d, rules)))
         out.append((t, d))
-    out.sort(key=lambda x: (-x[0], x[1]))
+    from stract_b200.bm25 import total_order_key
+    out.sort(key=lambda x: (-int(total_order_key(x[0])[0]), x[1]))   # total_cmp with the library's NaN rule (DESIGN §5)
     return out[:k]

@@ -59,3 +59,38 @@ def test_harvest_over_top_k_equals_harvest_over_everything():
         want = full.into_sorted_vec(True)
         got, K, proven = harvest_top_k(top_n, search, lambda d: hashes[d], k_max=8192)
         assert proven and got == want, (trial, K)
+
+
+def test_total_cmp_order_of_negative_zero_and_infinite_scores():
+    """ScoredDoc::cmp is f64::total_cmp (top_docs.rs:229-233): -0.0 pops after +0.0, -inf last, +inf first"""
+    scores = [-1.5, 0.0, -0.0, np.inf, -np.inf, 2.0, -3.0, 5e-324, -5e-324]
+    docs = [((i + 1, 100 + i, 200 + i, 300 + i, 0), i, s) for i, s in enumerate(scores)]
+    got = [s for s, _ in run(len(scores), docs)]
+    want = [np.inf, 2.0, 5e-324, 0.0, -0.0, -5e-324, -1.5, -3.0, -np.inf]
+    assert [np.float64(x).view(np.uint64) for x in got] == [np.float64(x).view(np.uint64) for x in want]
+
+
+def test_negative_scores_are_de_ranked_by_the_adjuster():
+    """the penalty divides the score, so a negative score moves UP towards 0 when its site was picked, as in the reference"""
+    c = BucketCollector(3, CollectorConfig())
+    for site, doc, score in ((1, 0, 0.5), (1, 1, -0.9), (2, 2, -0.95)):
+        c.insert(score, Hashes(site, 10 + doc, 20 + doc, 30 + doc, 0), doc)
+    got = c.into_sorted_vec(True, with_adjusted=True)
+    assert [d for d, _ in got] == [0, 1, 2] and got[1][1] == -0.9 * (1.0 / 1.1) and got[2][1] == -0.95
+
+
+def test_nan_scores_rank_by_their_bits_and_terminate():
+    """a positive NaN pops before +inf, a negative NaN after -inf; and after a pick the loop that re-adjusts the best
+    document meets a NaN at the top (the second positive NaN) and ends, because it compares bits -- the reference's `==`
+    never holds for a NaN and would loop forever"""
+    import struct
+    import threading
+    pos = struct.unpack("<d", struct.pack("<Q", 0x7FF8000000000000))[0]
+    neg = struct.unpack("<d", struct.pack("<Q", 0xFFF8000000000000))[0]
+    docs = [((1, 10, 20, 30, 0), 0, neg), ((1, 11, 21, 31, 0), 1, 1.0), ((2, 12, 22, 32, 0), 2, pos), ((3, 13, 23, 33, 0), 3, -np.inf),
+            ((4, 14, 24, 34, 0), 4, np.inf), ((5, 15, 25, 35, 0), 5, pos)]
+    out = []
+    t = threading.Thread(target=lambda: out.append(run(6, docs)), daemon=True)
+    t.start(); t.join(30)
+    assert out, "the collector did not terminate on a NaN best document"
+    assert [d for _, d in out[0]] == [2, 5, 4, 1, 3, 0]
