@@ -235,6 +235,17 @@ SB200_API int sb200_graph_distances(sb200_graph* g, const uint64_t* src_lo, cons
 SB200_API int sb200_approx_harmonic(sb200_graph* g, const uint64_t* src_lo, const uint64_t* src_hi, uint32_t n_sources,
                                     uint32_t max_dist, uint64_t num_nodes, uint64_t* id_lo, uint64_t* id_hi, double* centrality,
                                     uint64_t cap, uint64_t* len);
+/* Betweenness::calculate (crates/core/src/webgraph/centrality/betweenness.rs:29-146) for the caller's sources, in the given
+ * order (the reference takes the first 100 000 of an FxHashSet): Brandes' algorithm, one forward search per source over
+ * every kept link, sigma counted in i32 that wraps like the reference's release build, then
+ *     delta[v] = delta[v] + (sigma[v] as f64 / sigma[w] as f64) * (1.0 + delta[w])
+ * over v's successors w on the shortest-path DAG in ascending node id, and centrality[w] += delta[w] (w != source) in source
+ * order; the result is centrality / (n * (n - 1.0)), n = n_sources (n == 1 divides by zero, as in the reference).
+ * Output: every source and every node a source reaches, ascending id, at most n_nodes entries; max_dist = the largest
+ * distance of any search.  Refused: a source id that is not a node or repeats an earlier one, cap < n_nodes (SB200_EINVAL),
+ * a distance of 255 or more (SB200_ERANGE: distances are u8).  Single-rank handles. */
+SB200_API int sb200_betweenness(sb200_graph* g, const uint64_t* src_lo, const uint64_t* src_hi, uint32_t n_sources, uint64_t* id_lo,
+                                uint64_t* id_hi, double* centrality, uint64_t cap, uint64_t* len, uint32_t* max_dist);
 
 /* Inbound similarity (crates/core/src/ranking/inbound_similarity.rs:71-119 over bitvec_similarity.rs:130-185): for every
  * candidate node, Scorer::score against the liked / disliked nodes:

@@ -91,6 +91,8 @@ def declare(L):
     f("sb200_hyperball_state_bytes", i32, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64))
     f("sb200_hyperball_bind_state", i32, vp, vp, vp, vp, vp)
     f("sb200_hyperball_set_publish_targets", i32, vp, i32, vp, vp, vp, vp)
+    if hasattr(L, "sb200_betweenness"):   # absent from the CPU emulator library of the HyperBall / BM25 tests
+        f("sb200_betweenness", i32, vp, vp, vp, u32, vp, vp, vp, u64, C.POINTER(u64), C.POINTER(u32))
     try:
         from . import _lib_bm25
         _lib_bm25.proto(L, f)

@@ -15,6 +15,8 @@
 #pragma once
 #include "common.cuh"
 
+#include <vector>
+
 namespace sb200 {
 constexpr int MAX_PEERS = 15;
 // publish targets of a sharded handle, by value in the kernel parameters.  `sub` (nullable) is the subscriber mask
@@ -124,4 +126,24 @@ constexpr int CHUNK_EDGES = 1024;  // longer rows are cut into warp-sized work i
 int build_fwd_csr(sb200_graph* g);
 int stage_graph(sb200_graph* g, const uint64_t* from_lo, const uint64_t* from_hi, const uint64_t* to_lo,
                 const uint64_t* to_hi, const uint64_t* rel, uint64_t n_edges, uint64_t mask);
+__global__ void k_offsets_from_sorted(const uint64_t* keys, uint64_t n, uint64_t n_rows, uint32_t* ptr);
+
+// bit-parallel searches (graph_bfs.cu), shared with the betweenness passes (graph_betweenness.cu)
+struct BfsState {
+  DevBuf<unsigned long long> frontier, next, visited, any;
+  DevBuf<uint32_t> seed_rank, seed_bit;
+};
+// allocates the search words of `st` and maps the source ids to ranks (0xFFFFFFFF: not a node); single-rank handles
+int bfs_prepare(sb200_graph* g, BfsState& st, const uint64_t* src_lo, const uint64_t* src_hi, uint32_t n_sources, std::vector<uint32_t>& ranks);
+__global__ void k_bfs_seed(const uint32_t* seed_rank, const uint32_t* seed_bit, uint32_t n, const uint32_t* inv,
+                           unsigned long long* frontier, unsigned long long* visited);
+__global__ void __launch_bounds__(256) k_bfs_pull_items(uint64_t n_items, const uint32_t* item_row, const uint32_t* item_start,
+    uint32_t warp_row_begin, const uint32_t* row_ptr, const uint32_t* col, const unsigned long long* frontier, unsigned long long* next);
+__global__ void k_bfs_pull_rows(uint64_t row_begin, uint64_t row_end, const uint32_t* row_ptr, const uint32_t* col,
+                                const unsigned long long* frontier, unsigned long long* next);
+__global__ void k_bfs_commit(uint64_t N, const uint32_t* perm, unsigned long long* next, unsigned long long* visited,
+                             unsigned long long* frontier, uint32_t level, uint8_t* dist_out, uint32_t n_bits, double* cent, double term,
+                             unsigned long long* any);
+__global__ void k_ah_scatter(const uint32_t* flag, const uint32_t* pos, const double* val, const uint64_t* id_lo, const uint64_t* id_hi,
+                             uint64_t N, uint64_t cap, uint64_t* out_lo, uint64_t* out_hi, double* out_c);
 }  // namespace sb200

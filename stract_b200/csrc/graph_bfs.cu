@@ -138,11 +138,6 @@ __global__ void k_ah_scatter(const uint32_t* __restrict__ flag, const uint32_t* 
   out_lo[p] = id_lo[r]; out_hi[p] = id_hi[r]; out_c[p] = val[r];
 }
 
-struct BfsState {
-  DevBuf<unsigned long long> frontier, next, visited, any;
-  DevBuf<uint32_t> seed_rank, seed_bit;
-};
-
 // one batch of <= 64 searches; levels 1 .. max_level are committed (max_level == 0: until no search makes progress)
 static int bfs_batch(sb200_graph* g, BfsState& st, uint32_t n_seeds, uint32_t n_bits, uint32_t max_level, bool reversed, uint8_t* dist_dev,
                      double* cent, const std::vector<double>& term_of_level) {
@@ -178,7 +173,7 @@ static int bfs_batch(sb200_graph* g, BfsState& st, uint32_t n_seeds, uint32_t n_
   return SB200_OK;
 }
 
-static int bfs_prepare(sb200_graph* g, BfsState& st, const uint64_t* src_lo, const uint64_t* src_hi, uint32_t n_sources, std::vector<uint32_t>& ranks) {
+int bfs_prepare(sb200_graph* g, BfsState& st, const uint64_t* src_lo, const uint64_t* src_hi, uint32_t n_sources, std::vector<uint32_t>& ranks) {
   cudaStream_t s = g->stream;
   if (g->world != 1) SB_FAIL(SB200_ESTATE, "graph searches run on single-rank handles");
   const uint64_t N = g->N;

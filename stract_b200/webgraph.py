@@ -6,6 +6,7 @@ Mirrors (same names / argument meaning / behaviour):
                                   crates/core/src/webgraph/{edge.rs:30-35,mod.rs:157-194}
   HarmonicCentrality.calculate/get/iter/len
                                   crates/core/src/webgraph/centrality/harmonic.rs:289-311
+  Betweenness.calculate           crates/core/src/webgraph/centrality/betweenness.rs:29-175
   ShardedHarmonicCentrality       the AMPC job (entrypoint/ampc/harmonic_centrality/*): one process
                                   per GPU, the DHT max-upsert replaced by an all-gather of owned rows
 
@@ -329,6 +330,19 @@ class DeviceGraph:
         k = ln.value
         return olo[:k], ohi[:k], oc[:k]
 
+    def betweenness(self, sources):
+        """Betweenness::calculate for the given sources, in the given order (webgraph/centrality/betweenness.rs:29-146):
+        (ids_lo, ids_hi, centrality, max_dist) over the sources and the nodes they reach, in ascending id order.  Create the
+        handle with skipped_rel=0: the reference's ForwardlinksQuery sees every link."""
+        n = self.info()["n_nodes"]
+        lo = np.array([int(x) & _M64 for x in sources], np.uint64); hi = np.array([int(x) >> 64 for x in sources], np.uint64)
+        ln = C.c_uint64(0); md = C.c_uint32(0)
+        olo = host_out(n, np.uint64); ohi = host_out(n, np.uint64); oc = host_out(n, np.float64)
+        check(self._L.sb200_betweenness(self._h, lo.ctypes.data, hi.ctypes.data, len(lo), olo.ctypes.data if n else None,
+                                        ohi.ctypes.data if n else None, oc.ctypes.data if n else None, n, C.byref(ln), C.byref(md)))
+        k = ln.value
+        return olo[:k], ohi[:k], oc[:k], md.value
+
     def inbound_similarity(self, liked, disliked, candidates, normalized=False, self_score=1.0):
         """inbound_similarity::Scorer over the resident graph (ranking/inbound_similarity.rs:71-119): one f64 score per candidate."""
         def split(ids):
@@ -457,6 +471,29 @@ class HarmonicCentrality:
 
     def is_empty(self):
         return len(self.values) == 0
+
+
+class Betweenness:
+    """`Betweenness { centrality: HashMap<Node, f64>, max_dist }` (webgraph/centrality/betweenness.rs:149-175).
+
+    The reference takes the first 100 000 nodes of an FxHashSet as sources; here `sources=None` means every node when the
+    graph has at most MAX_SOURCES of them (the reference's source set), otherwise the first MAX_SOURCES in ascending id."""
+    MAX_SOURCES = 100_000
+
+    def __init__(self, ids_lo, ids_hi, values, max_dist):
+        self.ids_lo, self.ids_hi, self.values, self.max_dist = ids_lo, ids_hi, values, max_dist
+        self.centrality = {(int(h) << 64) | int(l): float(v) for l, h, v in zip(ids_lo, ids_hi, values)}
+
+    @classmethod
+    def calculate(cls, graph, device=0, sources=None):
+        dg = DeviceGraph(graph, device=device, skipped_rel=0)   # ForwardlinksQuery applies no rel-flag filter
+        try:
+            if sources is None:
+                lo, hi = dg.node_ids()
+                sources = [(int(h) << 64) | int(l) for l, h in zip(lo[:cls.MAX_SOURCES], hi[:cls.MAX_SOURCES])]
+            return cls(*dg.betweenness(sources))
+        finally:
+            dg.close()
 
 
 def run_sharded_loop(engine, world_size, group=None, max_iters=0):
