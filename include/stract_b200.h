@@ -266,8 +266,9 @@ SB200_API int sb200_inbound_similarity(sb200_graph* g, const uint64_t* liked_lo,
 /* Tuning switches of one handle: "quad_side_ctas" (CTAs per SM of the short-row kernel on the side stream of the fused
  * exchange, 0 = one stream; default 2 with up to 4 ranks or one multicast target, else 0), "owned_items" (0 / 1: launch the
  * long-row kernel over the owned work items only; default 1), "publish_all" (0 / 1: store produced rows into every peer, no
- * subscriber filter; default 0).  All ranks of a sharded computation must use the same "publish_all".  Not while an
- * iteration is in flight. */
+ * subscriber filter; default 0), "l2_window_mb" (size of the persisting L2 window over the head of the register array, 0..1024 MiB,
+ * capped by the device; 0 = no window; default 16).  All ranks of a sharded computation must use the same "publish_all".
+ * Not while an iteration is in flight. */
 SB200_API int sb200_hyperball_set_option(sb200_graph* g, const char* name, double value);
 
 /* Device-memory arena diagnostics.  With SB200_ARENA=1 in the environment, staging temporaries, the CSR and the

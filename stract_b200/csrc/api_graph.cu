@@ -15,6 +15,7 @@ void set_error(const char* fmt, ...) {
 }
 int hb_alloc_state(sb200_graph* g);
 int hb_reset(sb200_graph* g);
+int hb_set_l2_window(sb200_graph* g, uint64_t want);
 int hb_step(sb200_graph* g, sb200_iter_stats* st);
 int hb_step_launch(sb200_graph* g, bool with_barrier);
 int hb_step_finish(sb200_graph* g, sb200_iter_stats* st);
@@ -151,6 +152,11 @@ int sb200_hyperball_set_option(sb200_graph* g, const char* name, double value) {
   if (!strcmp(name, "quad_side_ctas")) { if (value < 0 || value > 16) SB_FAIL(SB200_EINVAL, "quad_side_ctas must be 0..16"); g->opt_side_ctas = (int)value; }
   else if (!strcmp(name, "owned_items")) g->opt_owned_list = value != 0.0 ? 1 : 0;
   else if (!strcmp(name, "publish_all")) g->publish_all = value != 0.0;
+  else if (!strcmp(name, "l2_window_mb")) {
+    if (!(value >= 0 && value <= 1024)) SB_FAIL(SB200_EINVAL, "l2_window_mb must be 0..1024");
+    SB_CUDA(cudaSetDevice(g->device));   // the persisting set-aside is a setting of the handle's device
+    SB_TRY(sb200::hb_set_l2_window(g, (uint64_t)(value * (1 << 20))));
+  }
   else SB_FAIL(SB200_EINVAL, "unknown option '%s'", name);
   return SB200_OK;
 }

@@ -139,28 +139,26 @@ __device__ __forceinline__ uint4 seed_slice(uint32_t s, uint32_t sub) {
   const uint32_t w = (j >> 2) & 3u;
   return make_uint4(w == 0u ? v : 0u, w == 1u ? v : 0u, w == 2u ? v : 0u, w == 3u ? v : 0u);
 }
+// One quad of lanes per node: lane q stores the 16-B slice q of both register rows, so that a warp writes 8 whole rows (512 B)
+// per store instruction.  size() of a freshly seeded counter needs no register sum: with one non-zero register, zeros = 63
+// and linear counting decides (h = lc[63] = 64 ln(64/63) = 1.008 is below the threshold 40, the `pick` of hll64_size), so
+// it is (usize) lc[63] = 1 for every node.
 __global__ void k_hb_init(const uint64_t* __restrict__ id_lo, const uint32_t* __restrict__ perm, uint64_t N,
                           uint4* r0, uint4* r1, uint16_t* seed, uint64_t* size_cache, double* ksum, double* kerr) {
-  __shared__ HllTables tab;
-  for (int i = threadIdx.x; i < (int)(sizeof(HllTables) / 8); i += blockDim.x) ((double*)&tab)[i] = ((const double*)&c_tab)[i];
-  __syncthreads();
-  uint64_t v = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const uint64_t v = gt >> 2;
+  const uint32_t q = (uint32_t)gt & 3u;
   if (v >= N) return;
   const uint64_t hash = id_lo[perm[v]] * 11400714819323198549ull;  // FastHasher hyperloglog.rs:4311-4313
   const uint32_t j = (uint32_t)(hash >> 58);
   const uint64_t wv = hash << 6;
   const uint32_t p = (wv == 0 ? 64u : (uint32_t)__clzll((long long)wv)) + 1u;
   const uint32_t s = j | p << 8;
-  seed[v] = (uint16_t)s;
-  uint32_t w[16];
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    const uint4 x = seed_slice(s, (uint32_t)q);
-    r0[v * 4 + q] = x; r1[v * 4 + q] = x;
-    w[4 * q] = x.x; w[4 * q + 1] = x.y; w[4 * q + 2] = x.z; w[4 * q + 3] = x.w;
-  }
-  size_cache[v] = hll64_size(w, &tab);
-  ksum[v] = 0.0; kerr[v] = 0.0;
+  const uint4 x = seed_slice(s, q);
+  r0[v * 4 + q] = x; r1[v * 4 + q] = x;
+  if (q == 0) { seed[v] = (uint16_t)s; size_cache[v] = (uint64_t)__double2ull_rz(c_tab.lc[63]); }
+  else if (q == 1) ksum[v] = 0.0;
+  else if (q == 2) kerr[v] = 0.0;
 }
 __global__ void k_bm_fill(uint32_t* bm, uint64_t N, uint64_t words) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -655,8 +653,13 @@ __global__ void k_gather_f64x2(const uint32_t* __restrict__ inv, const double* _
 // The seed iteration (t = 0) points the window at the seed array instead, capped at the same size.  Iteration 0 of C2
 // (28.8 MB of seeds), same card: no window 6.87, 16 MB 6.93, the whole array (a 30 MB window) 6.18 ms -- but a
 // 30 MB set-aside slows the dense iterations from 8.4 to 10.3 ms, so the cap stays.
+// Re-timed with tools/dense_iter_sweep.py (H100 80 GB at 700 W, ms per computation): 16 MB 39.11, 20 MB 39.00, 24 MB 39.60 --
+// 20 MB is inside the spread of 16 MB, so 16 MB stays.  Evict-first L2 hints on the pulls' read-once traffic (col, row_ptr,
+// own rows, new-row stores) changed none of these by more than the spread (DESIGN section 6), so the pulls carry none.
 constexpr uint64_t L2_WINDOW_BYTES = 16ull << 20;
+constexpr uint64_t SEED_WINDOW_BYTES = 16ull << 20;   // the cap of the seed iteration's window, whatever the pulls' window
 
+int hb_set_l2_window(sb200_graph* g, uint64_t want);
 int hb_alloc_state(sb200_graph* g) {
   const uint64_t N = g->N;
   const uint64_t words = (N + 31) / 32;
@@ -673,14 +676,29 @@ int hb_alloc_state(sb200_graph* g) {
     SB_CUDA(cudaMemset(g->sync_page.p, 0, SYNC_SLOTS * sizeof(unsigned long long)));
   }
   if (!g->h_counters) SB_CUDA(cudaMallocHost((void**)&g->h_counters, 8 * sizeof(unsigned long long)));
+  return hb_set_l2_window(g, L2_WINDOW_BYTES);
+}
+
+static int set_l2_window(cudaStream_t s, const void* base, uint64_t bytes);
+// the persisting window of the pulls: `want` bytes, capped by the device and the register array (0: no window).  The caller
+// has made g->device current.
+int hb_set_l2_window(sb200_graph* g, uint64_t want) {
   cudaDeviceProp prop;
   SB_CUDA(cudaGetDeviceProperties(&prop, g->device));
-  uint64_t want = L2_WINDOW_BYTES;
   want = std::min<uint64_t>(want, (uint64_t)std::max(prop.persistingL2CacheMaxSize, 0));
   want = std::min<uint64_t>(want, (uint64_t)std::max(prop.accessPolicyMaxWindowSize, 0));
-  want = std::min<uint64_t>(want, N * 64);
+  want = std::min<uint64_t>(want, g->N * 64);
+  const bool had = g->l2_window_bytes != 0;
   g->l2_window_bytes = 0;
-  if (want) { SB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want)); g->l2_window_bytes = want; }
+  if (want) { SB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want)); g->l2_window_bytes = want; return SB200_OK; }
+  if (had) {
+    // no window any more: the pulls stop re-pointing one (hb_step_launch), so drop the one the last pull left on each stream,
+    // give the set-aside back and turn the lines already pinned into normal ones
+    SB_TRY(set_l2_window(g->stream, nullptr, 0));
+    if (g->side_stream) SB_TRY(set_l2_window(g->side_stream, nullptr, 0));
+    SB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 0));
+    SB_CUDA(cudaCtxResetPersistingL2Cache());
+  }
   return SB200_OK;
 }
 
@@ -690,7 +708,7 @@ int hb_reset(sb200_graph* g) {
   g->cur = 0; g->bcur = 0; g->t = 0; g->has_changes = N > 0; g->exchange_pending = false;
   g->n_changed_prev = N; g->frontier_edges_prev = g->E_kept;
   if (N == 0) return SB200_OK;
-  SB_LAUNCH(k_hb_init, div_up(N, 256), 256, 0, s, g->id_lo.p, g->perm.p, N, (uint4*)g->regs[0].p, (uint4*)g->regs[1].p,
+  SB_LAUNCH(k_hb_init, div_up(N * 4, 256), 256, 0, s, g->id_lo.p, g->perm.p, N, (uint4*)g->regs[0].p, (uint4*)g->regs[1].p,
             g->seed.p, g->size_cache.p, g->kahan_sum.p, g->kahan_err.p);
   SB_CHECK_LAUNCH();
   SB_LAUNCH(k_bm_fill, div_up(words, 256), 256, 0, s, g->bm[0].p, N, words);  // changed_nodes filled, harmonic.rs:223-225
@@ -720,7 +738,7 @@ static PeerOut make_peer_out(const sb200_graph* g, bool with_targets) {
   return po;
 }
 
-// persisting-L2 access-policy window of the pull kernels on stream `s` (see hb_alloc_state)
+// persisting-L2 access-policy window of the pull kernels on stream `s` (see hb_alloc_state); 0 bytes: none
 static int set_l2_window(cudaStream_t s, const void* base, uint64_t bytes) {
   cudaStreamAttrValue a;
   memset(&a, 0, sizeof(a));
@@ -733,7 +751,8 @@ static int set_l2_window(cudaStream_t s, const void* base, uint64_t bytes) {
 // the window of a pull: the head of the `old` array, or in the seed iteration the head of the seed array
 static void l2_window_of(const sb200_graph* g, const uint4* oldr, bool from_seed, const void** base, uint64_t* bytes) {
   *base = from_seed ? (const void*)g->seed.p : (const void*)oldr;
-  *bytes = from_seed ? std::min<uint64_t>(g->l2_window_bytes, g->N * sizeof(uint16_t)) : g->l2_window_bytes;
+  *bytes = from_seed ? std::min<uint64_t>(std::min<uint64_t>(g->l2_window_bytes, SEED_WINDOW_BYTES), g->N * sizeof(uint16_t))
+                     : g->l2_window_bytes;
 }
 
 template <bool FRONTIER, bool SEED>

@@ -137,7 +137,8 @@ class DeviceGraph:
         check(self._L.sb200_hyperball_reset(self._h))
 
     def set_option(self, name, value):
-        """Tuning switch of this handle: "quad_side_ctas", "owned_items", "publish_all" (sb200_hyperball_set_option)."""
+        """Tuning switch of this handle: "quad_side_ctas", "owned_items", "publish_all", "l2_window_mb" (the persisting L2
+        window over the head of the register array, in MiB; 0 turns it off) (sb200_hyperball_set_option)."""
         check(self._L.sb200_hyperball_set_option(self._h, name.encode(), float(value)))
 
     def set_policy(self, dense_frac=-1.0, push_div=-1.0, force_mode=-1):
