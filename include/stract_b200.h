@@ -267,7 +267,9 @@ SB200_API int sb200_inbound_similarity(sb200_graph* g, const uint64_t* liked_lo,
  * exchange, 0 = one stream; default 2 with up to 4 ranks or one multicast target, else 0), "owned_items" (0 / 1: launch the
  * long-row kernel over the owned work items only; default 1), "publish_all" (0 / 1: store produced rows into every peer, no
  * subscriber filter; default 0), "l2_window_mb" (size of the persisting L2 window over the head of the register array, 0..1024 MiB,
- * capped by the device; 0 = no window; default 16).  All ranks of a sharded computation must use the same "publish_all".
+ * capped by the device; 0 = no window; default 16), "l1_hub_kb" (L1 budget of the pulls' hub sources, 0..2^30 KiB: the first
+ * kb * 1024 / 64 rows are gathered through L1 and every other source around it; 0 = no gather through L1, at least
+ * N * 64 / 1024 = every gather through L1; default: every gather through L1).  All ranks of a sharded computation must use the same "publish_all".
  * Not while an iteration is in flight. */
 SB200_API int sb200_hyperball_set_option(sb200_graph* g, const char* name, double value);
 

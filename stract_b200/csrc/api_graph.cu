@@ -157,6 +157,11 @@ int sb200_hyperball_set_option(sb200_graph* g, const char* name, double value) {
     SB_CUDA(cudaSetDevice(g->device));   // the persisting set-aside is a setting of the handle's device
     SB_TRY(sb200::hb_set_l2_window(g, (uint64_t)(value * (1 << 20))));
   }
+  else if (!strcmp(name, "l1_hub_kb")) {
+    // 0: every gather bypasses L1; at least N * 64 / 1024: every gather goes through L1
+    if (!(value >= 0 && value <= 1073741824.0)) SB_FAIL(SB200_EINVAL, "l1_hub_kb must be 0..1073741824");
+    g->l1_hub_bytes = (uint64_t)(value * 1024);
+  }
   else SB_FAIL(SB200_EINVAL, "unknown option '%s'", name);
   return SB200_OK;
 }

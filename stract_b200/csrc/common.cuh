@@ -186,4 +186,32 @@ __device__ __forceinline__ uint32_t ld_stream_u32(const uint32_t* p) {
 #endif
 }
 
+// 16-B loads of data that no thread writes during the launch (`.nc`, the read-only path).
+// ld_stream_u4: read once, do not allocate in L1.
+// ld_gather_u4: a gathered register slice.  A hub (hub = true) is kept in L1 with evict_last; any other source does not
+// allocate in L1, so the random tail of the gathers cannot evict the hubs.  The choice is a predicate on the two loads,
+// not a branch, so a warp's gathers stay in flight together whatever mix of hubs its lanes hold.
+__device__ __forceinline__ uint4 ld_stream_u4(const uint4* p) {
+#ifndef SB200_EMU
+  uint4 v;
+  asm("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
+#else
+  return *p;
+#endif
+}
+__device__ __forceinline__ uint4 ld_gather_u4(const uint4* p, bool hub) {
+#ifndef SB200_EMU
+  uint4 v = make_uint4(0, 0, 0, 0);
+  asm("{\n\t.reg .pred h;\n\tsetp.ne.u32 h, %5, 0;\n\t"
+      "@h ld.global.nc.L1::evict_last.v4.u32 {%0, %1, %2, %3}, [%4];\n\t"
+      "@!h ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];\n\t}"
+      : "+r"(v.x), "+r"(v.y), "+r"(v.z), "+r"(v.w) : "l"(p), "r"((uint32_t)hub));
+  return v;
+#else
+  (void)hub;
+  return *p;
+#endif
+}
+
 }  // namespace sb200

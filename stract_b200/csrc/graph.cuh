@@ -92,6 +92,10 @@ struct sb200_graph {
   double dense_frac = 0.35, push_div = 48.0;  // mode policy (see hb_step)
   int force_mode = -1;
   uint64_t l2_window_bytes = 0;  // persisting-L2 access window over the hot prefix of the `old` register array (hb_alloc_state)
+  // L1 budget of the pulls' hub sources: the first l1_hub_bytes / 64 rows are gathered through L1 with evict_last, all
+  // others around it (hyperball.cu, launch_pull; set_option "l1_hub_kb").  Default: every row (no budget below that was
+  // faster at C2, DESIGN section 6)
+  uint64_t l1_hub_bytes = UINT64_MAX;
 
   // optional per-kernel-family device timing (bench evidence; CUDA events on this handle's stream)
   enum { F_PULL_WARP_DENSE, F_PULL_QUAD_DENSE, F_PULL_WARP_FRONT, F_PULL_QUAD_FRONT, F_PULL_MERGE, F_PUSH, F_FINALIZE,

@@ -23,6 +23,9 @@
 //                     the 8 quads; rows spanning several items go through a partial buffer + k_pull_merge
 //     DENSE variant gathers every in-neighbour; FRONTIER variant tests the changed bitmap first; SEED variant (iteration
 //     0) gathers every in-neighbour's 2-B seed instead of its 64-B row: a reset counter has one non-zero register.
+//     Every gather of a source below the L1 hub budget (the highest in-degrees: rows are numbered by in-degree) goes
+//     through L1 with evict_last, every other one around L1 (ld_gather_u4).  The default budget is every row: at C2 no
+//     smaller budget was faster (DESIGN section 6).
 //   * push kernel (source-major CSR) for small frontiers: the frontier's out-edges in equal contiguous tiles per warp,
 //     half-warp per out-edge, 32-bit CAS max.
 //   * k_finalize: per changed node, HyperLogLog<64>::size() in the reference's exact f64 operation
@@ -53,6 +56,8 @@ struct HllTables {
 __constant__ HllTables c_tab;
 static bool g_tab_loaded[64] = {false};
 
+static int pulls_prefer_l1();
+// once per device: the HyperLogLog tables, and the pull kernels' cache configuration
 int load_tables(int device) {
   if (device >= 0 && device < 64 && g_tab_loaded[device]) return SB200_OK;
   static HllTables h;
@@ -60,6 +65,7 @@ int load_tables(int device) {
   h.lc[0] = 0.0;
   for (int v = 1; v <= 64; v++) h.lc[v] = 64.0 * std::log(64.0 / (double)v);  // hyperloglog.rs:4472-4476
   SB_CUDA(cudaMemcpyToSymbol(c_tab, &h, sizeof(h)));
+  SB_TRY(pulls_prefer_l1());
   if (device >= 0 && device < 64) g_tab_loaded[device] = true;
   return SB200_OK;
 }
@@ -201,18 +207,20 @@ __device__ __forceinline__ bool bm_test(const uint32_t* __restrict__ bm, uint32_
 // ---- pull, short rows: 4 lanes per destination row ----------------------------------------------------
 // SEED (iteration 0 only, see hb_step_launch): every row of `oldr` is the one-hot row of its seed, so the own row and
 // the sources are built from seed[] (2 B per source, L2-resident) and `oldr` is not read.
+// l1_hub: sources below it are hubs, gathered through L1 (ld_gather_u4); the SEED variant's cached 2-B loads ignore it.
 template <bool FRONTIER, bool SEED>
 __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub, uint32_t lane,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
-    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut& peers) {
+    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut& peers, uint32_t l1_hub) {
   static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
   const uint32_t e0 = live ? row_ptr[row] : 0u, e1 = live ? row_ptr[row + 1] : 0u;
-  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub) : oldr[row * 4 + sub];
+  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub)
+                         : ld_gather_u4(oldr + row * 4 + sub, row < l1_hub);
   uint4 acc = own;
   // lane `sub` fetches source index e+sub (one 16-B request per quad per 4 edges, prefetched one step ahead)
   // and the quad shares the four indices by shuffle; an out-of-range or (FRONTIER) unchanged source is
-  // redirected to the row itself, which is a no-op under max and hits L1.
+  // redirected to the row itself, which is a no-op under max.
   const unsigned qmask = 0xFu << (lane & ~3u);
   const uint32_t self = (uint32_t)row;
   uint32_t nxt = (e0 + sub < e1) ? ld_stream_u32(col + e0 + sub) : self;
@@ -241,10 +249,10 @@ __device__ __forceinline__ void quad_rows(uint64_t row, bool live, uint32_t sub,
     const uint32_t i1 = __shfl_sync(qmask, mine, 1, 4);
     const uint32_t i2 = __shfl_sync(qmask, mine, 2, 4);
     const uint32_t i3 = __shfl_sync(qmask, mine, 3, 4);
-    const uint4 v0 = oldr[(uint64_t)i0 * 4 + sub];
-    const uint4 v1 = oldr[(uint64_t)i1 * 4 + sub];
-    const uint4 v2 = oldr[(uint64_t)i2 * 4 + sub];
-    const uint4 v3 = oldr[(uint64_t)i3 * 4 + sub];
+    const uint4 v0 = ld_gather_u4(oldr + (uint64_t)i0 * 4 + sub, i0 < l1_hub);
+    const uint4 v1 = ld_gather_u4(oldr + (uint64_t)i1 * 4 + sub, i1 < l1_hub);
+    const uint4 v2 = ld_gather_u4(oldr + (uint64_t)i2 * 4 + sub, i2 < l1_hub);
+    const uint4 v3 = ld_gather_u4(oldr + (uint64_t)i3 * 4 + sub, i3 < l1_hub);
     acc = vmax_u8x16(vmax_u8x16(acc, v0), vmax_u8x16(vmax_u8x16(v1, v2), v3));
   }
   const unsigned ball = __ballot_sync(0xffffffffu, ne_u4(acc, own));
@@ -257,7 +265,7 @@ template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64_t row_end,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
-    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
+    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers, uint32_t l1_hub) {
   const uint64_t gt = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   const uint32_t sub = threadIdx.x & 3;
   const uint32_t lane = threadIdx.x & 31;
@@ -266,7 +274,7 @@ __global__ void __launch_bounds__(256, 7) k_pull_quad(uint64_t row_begin, uint64
   if (!live) row = row_end - 1;  // keep the warp converged; results of dead quads are discarded
   live = live && owned_row(peers, (uint32_t)row);
   if (__ballot_sync(0xffffffffu, live) == 0u) return;  // none of this warp's rows belongs to this rank
-  quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers);
+  quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers, l1_hub);
 }
 
 // Sharded handles with the fused exchange: the short rows are most of the rows, so this kernel carries most of the
@@ -277,7 +285,7 @@ template <bool FRONTIER, bool SEED>
 __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, uint64_t row_end, uint64_t first_block, uint64_t n_tasks,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr,
-    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
+    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers, uint32_t l1_hub) {
   const uint32_t sub = threadIdx.x & 3, lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
   for (uint64_t task = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; task < n_tasks; task += warps) {
@@ -286,7 +294,7 @@ __global__ void __launch_bounds__(256, 4) k_pull_quad_owned(uint64_t row_begin, 
     const bool live = row >= row_begin && row < row_end;
     if (!live) row = row_begin;
     if (__ballot_sync(0xffffffffu, live) == 0u) continue;
-    quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers);
+    quad_rows<FRONTIER, SEED>(row, live, sub, lane, row_ptr, col, oldr, seed, newr, bm_prev, bm_cur, peers, l1_hub);
   }
 }
 
@@ -298,7 +306,7 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
     const uint32_t* __restrict__ item_list, const uint32_t* __restrict__ item_row, const uint32_t* __restrict__ item_start, uint32_t warp_row_begin,
     const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
     const uint4* __restrict__ oldr, const uint16_t* __restrict__ seed, uint4* __restrict__ newr, uint4* __restrict__ partial,
-    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers) {
+    const uint32_t* __restrict__ bm_prev, uint32_t* __restrict__ bm_cur, const PeerOut peers, uint32_t l1_hub) {
   static_assert(!(FRONTIER && SEED), "the seed iteration gathers every source");
   uint64_t item = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
   if (item >= n_items) return;  // whole warp exits together
@@ -312,7 +320,7 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
   const uint32_t e1 = min(e0 + (uint32_t)CHUNK_EDGES, re);
   uint4 acc = make_uint4(0, 0, 0, 0);
   // out-of-range lanes and (FRONTIER) unchanged sources are redirected to the row itself: merging one's own row
-  // is a no-op under max and hits L1, so the gather loop is branch-free
+  // is a no-op under max, so the gather loop is branch-free
   uint32_t nxt = (e0 + lane < e1) ? ld_stream_u32(col + e0 + lane) : row;
   if (SEED) {
     // SEED (see quad_rows): each lane loads the 2-B seed of its source, one batch ahead, and the index one batch
@@ -339,10 +347,10 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
     const uint32_t i1 = __shfl_sync(0xffffffffu, mine, q + 8);
     const uint32_t i2 = __shfl_sync(0xffffffffu, mine, q + 16);
     const uint32_t i3 = __shfl_sync(0xffffffffu, mine, q + 24);
-    const uint4 v0 = oldr[(uint64_t)i0 * 4 + sub];
-    const uint4 v1 = oldr[(uint64_t)i1 * 4 + sub];
-    const uint4 v2 = oldr[(uint64_t)i2 * 4 + sub];
-    const uint4 v3 = oldr[(uint64_t)i3 * 4 + sub];
+    const uint4 v0 = ld_gather_u4(oldr + (uint64_t)i0 * 4 + sub, i0 < l1_hub);
+    const uint4 v1 = ld_gather_u4(oldr + (uint64_t)i1 * 4 + sub, i1 < l1_hub);
+    const uint4 v2 = ld_gather_u4(oldr + (uint64_t)i2 * 4 + sub, i2 < l1_hub);
+    const uint4 v3 = ld_gather_u4(oldr + (uint64_t)i3 * 4 + sub, i3 < l1_hub);
     acc = vmax_u8x16(vmax_u8x16(acc, v0), vmax_u8x16(vmax_u8x16(v1, v2), v3));
   }
 #pragma unroll
@@ -356,7 +364,8 @@ __global__ void __launch_bounds__(256, 8) k_pull_warp(uint64_t n_items, uint64_t
     if (q == 0) partial[item * 4 + sub] = acc;
     return;
   }
-  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub) : oldr[(uint64_t)row * 4 + sub];
+  const uint4 own = SEED ? seed_slice(__ldg(seed + row), sub)
+                         : ld_gather_u4(oldr + (uint64_t)row * 4 + sub, row < l1_hub);
   acc = vmax_u8x16(acc, own);
   const unsigned ball = __ballot_sync(0xffffffffu, ne_u4(acc, own));
   const bool changed = (ball & 0xFu) != 0u;
@@ -375,7 +384,7 @@ __global__ void __launch_bounds__(256) k_pull_merge(uint64_t n_rows, const uint3
   if (!owned_row(peers, row)) return;
   const uint32_t i0 = item_start[r], i1 = item_start[r + 1];
   uint4 acc = make_uint4(0, 0, 0, 0);
-  for (uint32_t it = i0 + q; it < i1; it += 8) acc = vmax_u8x16(acc, partial[(uint64_t)it * 4 + sub]);
+  for (uint32_t it = i0 + q; it < i1; it += 8) acc = vmax_u8x16(acc, ld_stream_u4(partial + (uint64_t)it * 4 + sub));
 #pragma unroll
   for (int off = 4; off < 32; off <<= 1) {
     uint4 o;
@@ -659,6 +668,24 @@ __global__ void k_gather_f64x2(const uint32_t* __restrict__ inv, const double* _
 constexpr uint64_t L2_WINDOW_BYTES = 16ull << 20;
 constexpr uint64_t SEED_WINDOW_BYTES = 16ull << 20;   // the cap of the seed iteration's window, whatever the pulls' window
 
+// The pulls keep their hub sources in L1 (ld_gather_u4).  None of them uses shared memory, so they prefer the largest L1
+// carve-out: the hubs are then not limited by a carve-out the driver picked.
+static int pulls_prefer_l1() {
+#ifndef SB200_EMU
+  const void* pulls[] = {
+      (const void*)k_pull_quad<false, false>, (const void*)k_pull_quad<true, false>, (const void*)k_pull_quad<false, true>,
+      (const void*)k_pull_quad_owned<false, false>, (const void*)k_pull_quad_owned<true, false>,
+      (const void*)k_pull_quad_owned<false, true>,
+      (const void*)k_pull_warp<false, false, false>, (const void*)k_pull_warp<true, false, false>,
+      (const void*)k_pull_warp<false, false, true>, (const void*)k_pull_warp<false, true, false>,
+      (const void*)k_pull_warp<true, true, false>, (const void*)k_pull_warp<false, true, true>,
+      (const void*)k_pull_merge};
+  for (const void* k : pulls)
+    SB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxL1));
+#endif
+  return SB200_OK;
+}
+
 int hb_set_l2_window(sb200_graph* g, uint64_t want);
 int hb_alloc_state(sb200_graph* g) {
   const uint64_t N = g->N;
@@ -772,6 +799,7 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
     g->opt_side_ctas = (multicast_target || g->world <= 4) ? 2 : 0;
   }
   const int side_ctas = g->opt_side_ctas;
+  const uint32_t l1_hub = (uint32_t)std::min<uint64_t>(g->l1_hub_bytes / 64, g->N);
   const bool side_quad = side_ctas > 0 && g->world > 1 && g->p2p && g->n_peers > 0 && g->n_items && g->quad_row_end > g->quad_row_begin;
   if (side_quad) {
     if (!g->side_stream) {
@@ -799,7 +827,7 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
       const unsigned grid = (unsigned)std::min<uint64_t>(div_up(n_tasks, 8), (uint64_t)sm_count * (uint64_t)side_ctas);
       auto kern = k_pull_quad_owned<FRONTIER, SEED>;
       SB_LAUNCH(kern, grid, 256, 0, g->side_stream, g->quad_row_begin, g->quad_row_end, first, n_tasks,
-                g->row_ptr.p, g->col.p, oldr, g->seed.p, newr, bmp, bmc, po);
+                g->row_ptr.p, g->col.p, oldr, g->seed.p, newr, bmp, bmc, po, l1_hub);
       SB_CHECK_LAUNCH();
     }
     if (g->profiling) {
@@ -816,7 +844,7 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
     if (n_launch)
     SB_LAUNCH(kern, div_up(n_launch * 32, 256), 256, 0, s, n_launch, g->n_multi_items,
               listed ? g->owned_items.p : (const uint32_t*)nullptr, g->item_row.p, g->item_start.p, (uint32_t)g->warp_row_begin, g->row_ptr.p, g->col.p, oldr,
-              g->seed.p, newr, g->partial.p, bmp, bmc, po);
+              g->seed.p, newr, g->partial.p, bmp, bmc, po, l1_hub);
     SB_CHECK_LAUNCH();
     PROF_END(g, FW, g->own_frac * (per_edge * (double)g->E_warp + 68.0 * (double)(g->warp_row_end - g->warp_row_begin - g->n_multi_rows)));
   }
@@ -833,7 +861,7 @@ static int launch_pull(sb200_graph* g, const uint4* oldr, uint4* newr, const uin
     PROF_BEGIN(g, FQ);
     auto kern = k_pull_quad<FRONTIER, SEED>;
     SB_LAUNCH(kern, div_up(nq * 4, 256), 256, 0, s, g->quad_row_begin, g->quad_row_end, g->row_ptr.p,
-              g->col.p, oldr, g->seed.p, newr, bmp, bmc, po);
+              g->col.p, oldr, g->seed.p, newr, bmp, bmc, po, l1_hub);
     SB_CHECK_LAUNCH();
     PROF_END(g, FQ, g->own_frac * (per_edge * (double)g->E_quad + 68.0 * (double)nq));
   }

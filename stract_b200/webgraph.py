@@ -138,7 +138,8 @@ class DeviceGraph:
 
     def set_option(self, name, value):
         """Tuning switch of this handle: "quad_side_ctas", "owned_items", "publish_all", "l2_window_mb" (the persisting L2
-        window over the head of the register array, in MiB; 0 turns it off) (sb200_hyperball_set_option)."""
+        window over the head of the register array, in MiB; 0 turns it off), "l1_hub_kb" (the pulls' L1 budget for hub
+        sources, in KiB; 0 sends every gather around L1) (sb200_hyperball_set_option)."""
         check(self._L.sb200_hyperball_set_option(self._h, name.encode(), float(value)))
 
     def set_policy(self, dense_frac=-1.0, push_div=-1.0, force_mode=-1):
